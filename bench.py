@@ -1,10 +1,10 @@
 #!/usr/bin/env python
-"""bench.py -- env-steps/sec of the PHC hot path (fused obs+reward+PPO) on N B200s of one node.
+"""bench.py -- env-steps/sec of the PHC hot path (fused obs+reward+PPO) on N H100s of one node.
 
     python bench.py --gpus 1 --steps 5 --warmup 3                (N > 1: launched by torchrun, one rank per GPU)
     python bench.py --impl reference ...                         (the reference algorithm's CPU port on the host cores)
 
-One "step" = one PPO epoch of the BASELINE.json configuration `4096 envs, 1xB200: fused obs+reward+GAE+PPO on synthetic
+One "step" = one PPO epoch of the BASELINE.json configuration `4096 envs, 1 GPU: fused obs+reward+GAE+PPO on synthetic
 24-body SMPL rigid-body state` PER GPU (weak scaling: every rank owns 4096 envs):
   32 rollout steps x [ simulator snapshot -> fused env step kernel (MotionLib query, self/task obs, reward, reset, AMP
   obs) -> masked reset path -> obs normalise -> actor + critic forward -> Gaussian sample -> critic on next obs ]
@@ -61,6 +61,7 @@ def parse_args():
     ap.add_argument("--no-points", action="store_true", help="skip the 16384 / 65536-env points of the env-step roofline")
     ap.add_argument("--workload", default="smpl", choices=sorted(WORKLOADS), help="configuration of the headline numbers (default: the one the metric is quoted on)")
     ap.add_argument("--no-extras", action="store_true", help="skip the secondary configurations (H1, PNN big nets) reported as extra_configs")
+    ap.add_argument("--dump-outputs", metavar="DIR", help="after the timed steps, write what the last timed epoch computed to DIR/<name>.npy")
     return ap.parse_args()
 
 
@@ -71,7 +72,7 @@ def measured_peak_gbs():
             return float(json.load(open(p))["hbm_gbs"]), "measured (MEASURED_PEAKS.json hbm_gbs)"
         except Exception:
             pass
-    return 6650.0, "fallback 6.65 TB/s (B200_PROFILING.md)"
+    return 3350.0, "fallback 3.35 TB/s (H100 SXM data sheet)"
 
 
 # ----------------------------------------------------------------------------------------------------------------
@@ -268,7 +269,7 @@ def run_reference_arm(args):
 
 
 # ----------------------------------------------------------------------------------------------------------------
-# the B200 arm
+# the GPU arm
 # ----------------------------------------------------------------------------------------------------------------
 WORKLOADS = {
     # BASELINE.json configs[1]: the configuration the metric is quoted on (and what the driver's default run measures)
@@ -288,6 +289,7 @@ def build_agent(num_envs: int, device, rank: int, world: int, host_bank: bool, w
     from phc_b200.env.humanoid_im import HumanoidIm, RLGPUEnv
     from phc_b200.learning.amp_agent import AMPAgent
     cfg = {"multi_gpu": world > 1, "seed": 0, "device": str(device)}
+    torch.manual_seed(rank)              # reset phases, policy noise, minibatch order: the same every run (the reference's set_seed)
     if workload == "h1":
         motion = syn.make_robot_motions(num_envs, seed=rank)
     else:
@@ -318,8 +320,9 @@ def timed_epochs(agent, steps: int, warmup: int, world: int, read_result: bool):
     lib = agent._lib
     l0 = lib.phc_launch_count()
     ev0.record()
+    result = None
     for _ in range(steps):
-        agent.train_epoch()
+        result = agent.train_epoch()
         if read_result:
             agent.train_result_dict()            # device->host read of the epoch's last losses (e2e mode)
     ev1.record()
@@ -332,7 +335,36 @@ def timed_epochs(agent, steps: int, warmup: int, world: int, read_result: bool):
         t = torch.tensor([ms], device=agent.device)
         torch.distributed.all_reduce(t, op=torch.distributed.ReduceOp.MAX)
         ms = float(t.item())
-    return ms / steps, launches
+    return ms / steps, launches, result
+
+
+DUMP_BUDGET_BYTES = 64 * 1024 * 1024   # all files together; an array over its even share is written as a fixed, seeded sample
+
+
+def dump_outputs(agent, result, out_dir: str) -> None:
+    """What the last timed epoch handed back (AMPAgent.train_epoch's tensors), the losses of its last minibatch and the network
+    parameters it left behind, one .npy per array: float32 (float64 for the losses).  The inputs are seeded, so two builds run
+    with the same arguments can be compared output for output."""
+    import numpy as np
+    os.makedirs(out_dir, exist_ok=True)
+    tensors = {k: v for k, v in result.items() if torch.is_tensor(v)}
+    tensors["params"] = agent.model.params
+    losses = agent.train_result_dict()
+    arrays = {"losses": np.array([losses[k] for k in sorted(losses)], dtype=np.float64)}
+    share = (DUMP_BUDGET_BYTES - arrays["losses"].nbytes) // 4 // len(tensors)      # float32 elements per array
+    for name, t in sorted(tensors.items()):
+        flat = t.detach().reshape(-1).float()
+        if flat.numel() > share:
+            idx = torch.randperm(flat.numel(), generator=torch.Generator().manual_seed(0))[:share].sort().values
+            arrays[name] = flat[idx.to(flat.device)].cpu().numpy()
+        else:
+            arrays[name] = flat.cpu().numpy().reshape(tuple(t.shape))
+    total = sum(a.nbytes for a in arrays.values())
+    if total > DUMP_BUDGET_BYTES:
+        raise RuntimeError(f"--dump-outputs: {total} bytes exceed the {DUMP_BUDGET_BYTES}-byte budget")
+    os.makedirs(out_dir, exist_ok=True)
+    for name, a in arrays.items():
+        np.save(os.path.join(out_dir, f"{name}.npy"), a)
 
 
 def env_kernel_roofline(task, peak_gbs: float, peak_src: str, iters: int = 40, algo_bytes: int = ALGO_BYTES_PER_ENV_STEP,
@@ -380,13 +412,7 @@ def env_kernel_roofline(task, peak_gbs: float, peak_src: str, iters: int = 40, a
     if not sane:
         t = t_pair
     N = task.num_envs
-    traffic = None            # DRAM bytes per launch from the committed ncu --set full capture of this kernel at this size
-    try:
-        tj = json.load(open(os.path.join(ROOT, "profiles", "env_step_traffic.json")))
-        if int(tj.get("num_envs", -1)) == N:
-            traffic = int(tj["dram_bytes_per_launch"])
-    except Exception:
-        traffic = None
+    traffic = None            # DRAM bytes per launch: not measured (needs a hardware-counter capture)
     achieved = algo_bytes * N / t / 1e9
     # what the launch really moves per env at J=24: inputs 1248 (state) + 1248 (cached reference pose of the reward time)
     # + 2 x 1248 (observation bracket) + 552 + 276 (dof) + 56 (scalars, env_motion); outputs 3744 (obs row incl. 8 pad bytes)
@@ -401,14 +427,14 @@ def env_kernel_roofline(task, peak_gbs: float, peak_src: str, iters: int = 40, a
             "peak_source": peak_src,
             "timing": "L2 flushed (torch fill_ of 256 MB) before each launch; kernel_us = (%d x [flush, kernel] - %d x [flush]) / %d, one "
                       "CUDA-event pair per batch, median of 5; the env step is a programmatic-dependent launch as everywhere in the product "
-                      "(PHC_ENV_PDL=0 gives the plain stream-ordered launch: +2.4 us at 4096 envs, profiles/ab_env_r2.log); "
+                      "(PHC_ENV_PDL=0 gives the plain stream-ordered launch); "
                       "kernel_us_event_pair = median of %d single launches, one event pair each" % (iters, iters, iters, iters)}
 
 
 def measured_peak_tf32():
     """Dense TF32 tensor peak to hold the 3xTF32 GEMMs against: MEASURED_PEAKS.json has no TF32 entry, so half of the measured
-    cuBLAS bf16 rate (kind::tf32 issues at half the kind::f16 rate: tcgen05 K = 8 vs 16 per instruction at the same cycle cost).
-    The sustained figure, because the GEMMs run back to back inside a long step (B200_PROFILING.md)."""
+    bf16 rate (wgmma tf32 issues K = 8 per instruction against K = 16 for bf16 at the same cycle cost).  The sustained figure,
+    because the GEMMs run back to back inside a long step."""
     p = os.path.join(ROOT, "MEASURED_PEAKS.json")
     if os.path.exists(p):
         try:
@@ -416,11 +442,11 @@ def measured_peak_tf32():
             return 0.5 * float(j["bf16_tflops_sustained"]), "0.5 x measured bf16_tflops_sustained (MEASURED_PEAKS.json); burst would be 0.5 x %.0f" % float(j["bf16_tflops"])
         except Exception:
             pass
-    return 0.5 * 1400.0, "0.5 x fallback 1.4 PFLOP/s sustained bf16 (B200_PROFILING.md)"
+    return 0.5 * 989.0, "0.5 x 989 TFLOP/s dense bf16 (H100 SXM data sheet)"
 
 
 def gemm_roofline(agent, iters: int = 20):
-    """Tensor-pipe roofline of the learner's dominant kernel (phc::tc5::smem_split::gemm_tc5s_kernel): the three grouped
+    """Tensor-pipe roofline of the learner's dominant kernel (phc::wg::gemm_wgmma_kernel): the three grouped
     forward launches of one minibatch (layer 1 / layer 2 / heads of actor + critic at 16384 rows and discriminator at 12288
     rows) and the grouped backward launches, timed back to back with CUDA events on the launching stream.  achieved = 3 x
     algorithmic fp32 FLOPs (3xTF32: three tensor-core products per fp32 product) / time."""
@@ -460,7 +486,7 @@ def gemm_roofline(agent, iters: int = 20):
     passes = 1.0 if eng.precision == "tf32" else 3.0          # tensor-core products per fp32 product
     ach = passes * (fl_f + fl_b) / (t_f + t_b) / 1e12
     return {"bound": "tensor", "achieved": ach, "peak": peak, "unit": "TFLOP/s", "frac": ach / peak, "traffic": None,
-            "kernel": "phc::tc5::smem_split::gemm_tc5s_kernel (grouped forward + backward launches of one minibatch)",
+            "kernel": "phc::wg::gemm_wgmma_kernel (grouped forward + backward launches of one minibatch)",
             "forward_us": t_f * 1e6, "forward_tflops": passes * fl_f / t_f / 1e12, "backward_us": t_b * 1e6,
             "backward_tflops": passes * fl_b / t_b / 1e12, "tensor_products_per_fp32_product": passes, "algorithmic_fp32_flops_per_minibatch": fl_f + fl_b,
             "fp32_equivalent_tflops": (fl_f + fl_b) / (t_f + t_b) / 1e12, "peak_source": src,
@@ -495,7 +521,7 @@ def run_extra_config(name: str, device, rank: int, world: int, peak_gbs: float, 
     w = WORKLOADS[name]
     try:
         agent, task = build_agent(w["envs"], device, rank, world, host_bank=False, workload=name)
-        ms, launches = timed_epochs(agent, steps, warmup, world, read_result=False)
+        ms, launches, _ = timed_epochs(agent, steps, warmup, world, read_result=False)
         out = {"workload": f"PPO epoch: {w['envs']} envs/GPU x 32 steps, {w['desc']}, minibatch 16384 x 6 mini-epochs", "num_envs_per_gpu": w["envs"],
                "value": HORIZON * w["envs"] * world / (ms * 1e-3), "unit": "env-steps/s", "ms_per_step": ms, "steps": steps, "warmup": warmup,
                "gpu_launches": int(launches), "dtype": "tf32 single pass (MLPs), f32 elsewhere" if name.endswith("_tf32") else "f32"}
@@ -543,8 +569,11 @@ def main():
     note("agent built; timed epochs")
     if rank == 0:
         sampler.start()
-    sec_per_step, launches = timed_epochs(agent, args.steps, args.warmup, world, read_result=False)
+    sec_per_step, launches, last = timed_epochs(agent, args.steps, args.warmup, world, read_result=False)
     clocks = sampler.stop() if rank == 0 else None
+    if args.dump_outputs and rank == 0:
+        dump_outputs(agent, last, args.dump_outputs)
+        note(f"outputs of the last timed epoch written to {args.dump_outputs}")
     note(f"value arm done: {sec_per_step:.1f} ms/epoch")
     if os.environ.get("PHC_PHASE_TIMING", "0") == "1" and rank == 0:       # diagnostic only: CUDA-event phase breakdown of one epoch
         agent.timer.report()
@@ -572,7 +601,7 @@ def main():
     if not args.no_e2e:
         agent2, task2 = build_agent(args.num_envs, device, rank, world, host_bank=True, workload=args.workload)
         note("e2e agent built (pinned host snapshots)")
-        ms2, _ = timed_epochs(agent2, max(1, args.steps), max(3, args.warmup) if args.warmup >= 3 else args.warmup, world, read_result=True)
+        ms2, _, _ = timed_epochs(agent2, max(1, args.steps), max(3, args.warmup) if args.warmup >= 3 else args.warmup, world, read_result=True)
         e2e = {"value": env_steps / (ms2 * 1e-3), "unit": "env-steps/s", "ms_per_step": ms2,
                "h2d_bytes_per_step": HORIZON * task2.sim.h2d_bytes_per_step, "d2h_bytes_per_step": 16 * 4,
                "note": "simulator state (rigid bodies, dof state, dof forces) copied from pinned host memory every env step; epoch losses read back"}
@@ -606,7 +635,7 @@ def main():
                 "dtype": "f32", "data": "synthetic",
                 "config": {"workload": workload_string(args.num_envs) if args.workload == "smpl" else f"PPO epoch: {args.num_envs} envs/GPU x 32 steps, {wl['desc']}, minibatch 16384 x 6 mini-epochs",
                            "parallelism": f"dp{world} (env shards, 1 NCCL all-reduce per minibatch)",
-                           "arithmetic": "fp32 throughout (the reference trains with mixed_precision: False): env kernels fp32, MLP GEMMs 3xTF32 on tcgen05 with fp32 accumulation",
+                           "arithmetic": "fp32 throughout (the reference trains with mixed_precision: False): env kernels fp32, MLP GEMMs 3xTF32 on wgmma with fp32 accumulation",
                            "l2": "inputs larger than L2: 2.1 GB experience buffer + ~1 GB frame tables per epoch; the roofline kernel is timed with an explicit L2 flush"},
                 "clocks": clocks, "e2e": e2e, "gpu_launches": int(launches), "roofline": roof, "roofline_gemm": roof_gemm, "cpu_baseline": cpu, "extra_configs": extras}
         print(json.dumps(line), flush=True)

@@ -1,4 +1,4 @@
-/* phc_b200 -- C ABI of the B200-native PHC hot path (libphc_b200.so).
+/* phc_b200 -- C ABI of the GPU-native PHC hot path (libphc_b200.so, built for the H100: sm_90a).
  *
  * The reference (ZhengyiLuo/PHC) has NO native boundary: the whole path is Python/TorchScript.  This header is
  * where one is cut.  Every entry point replaces a group of reference functions (cited file:line, relative to the
@@ -36,7 +36,7 @@ PHC_API int phc_version(void);
 PHC_API const char* phc_last_error(void);
 /* Number of CUDA kernels this library has launched in the calling process (monotonic; bench.py reports the delta). */
 PHC_API int64_t phc_launch_count(void);
-/* SM architecture the library was compiled for (100 for sm_100a). */
+/* SM architecture the library was compiled for (90 for sm_90a). */
 PHC_API int phc_compiled_sm(void);
 
 /* ------------------------------------------------------------------------------------------------------------
@@ -375,16 +375,16 @@ PHC_API int phc_adv_norm(const float* returns, const float* values, int64_t n, i
 PHC_API int phc_gemm(const float* A, int64_t lda, int32_t a_kmajor, const float* B, int64_t ldb, int32_t b_kmajor, float* C,
              int64_t ldc, int32_t M, int32_t N, int32_t K, float alpha, const float* bias, int32_t act,
              float* aux, int64_t ldaux, int32_t accumulate, int32_t k_splits, void* stream);
-/* Blackwell-native variant of phc_gemm: tcgen05.mma kind::tf32 (UMMA) fed by TMA, accumulator in TMEM.  Same epilogue
- * contract.  3xTF32 needs each operand pre-split once by phc_split_tf32 (hi = rna_tf32(x), lo = rna_tf32(x - hi)); hi and
- * lo share the leading dimension.  All four operand arrays 16-byte aligned, lda/ldb multiples of 4 (TMA strides). */
+/* Hopper tensor-core variant of phc_gemm (wgmma kind tf32, gemm_wgmma.cu).  Same epilogue contract.  3xTF32 with each
+ * operand pre-split once by phc_split_tf32 (hi = rna_tf32(x), lo = rna_tf32(x - hi)); hi and lo share the leading
+ * dimension.  All four operand arrays 16-byte aligned, lda/ldb multiples of 4; C 8-byte aligned, ldc even. */
 PHC_API int phc_split_tf32(const float* x, int64_t ldx, int64_t rows, int32_t cols, float* hi, float* lo, int64_t ldo, void* stream);
 PHC_API int phc_gemm_tc5(const float* A_hi, const float* A_lo, int64_t lda, int32_t a_kmajor, const float* B_hi, const float* B_lo,
                  int64_t ldb, int32_t b_kmajor, float* C, float* C_hi /* optional: split copies of C for the next GEMM */,
                  float* C_lo, int64_t ldc, int32_t M, int32_t N, int32_t K, float alpha, const float* bias, int32_t act,
                  float* aux, int64_t ldaux, int32_t accumulate, int32_t k_splits, void* stream);
-/* The same GEMM with the 3xTF32 operand split done in SHARED memory (gemm_tc5s.cu): plain fp32 operands, no pre-split
- * copies; TMA tensor stores (reduce-add for accumulate / split-K).  A, B, C 16-byte aligned; lda, ldb, ldc multiples of 4.
+/* The same GEMM with the 3xTF32 operand split done in SHARED memory (gemm_wgmma.cu): plain fp32 operands, no pre-split
+ * copies.  A, B, C 16-byte aligned; lda, ldb, ldc multiples of 4.
  * phc_gemm_group runs up to PHC_GEMM_GROUP_MAX independent problems (e.g. the same layer of actor, critic and
  * discriminator: network_builder.py:105-124 builds three separate nn.Sequential stacks that the reference evaluates one
  * after the other) as ONE persistent launch over the union of their tiles. */
@@ -399,10 +399,10 @@ typedef struct PhcGemmDesc {
   int32_t act;              /* PHC_ACT_* */
   float* aux; int64_t ldaux;
   int32_t accumulate, k_splits;
-  const float* B_lo;        /* optional: the 3xTF32 low part of B, same layout and ldb, made by phc_split_lo (weights: split once per
-                             * optimizer step instead of once per tile visit); NULL = the kernel splits B's tiles itself */
+  const float* B_lo;        /* optional: the 3xTF32 low part of B, same layout and ldb, made by phc_split_lo; validated and not
+                             * read (the kernel makes the identical low part from the tiles it stages) */
 } PhcGemmDesc;
-/* lo[i] = rna_tf32(x[i] - trunc_tf32(x[i])): the second TF32 term of every fp32 value, what the GEMM's splitter warps compute per tile */
+/* lo[i] = rna_tf32(x[i] - trunc_tf32(x[i])): the second TF32 term of every fp32 value, what the GEMM computes per staged tile */
 PHC_API int phc_split_lo(const float* x, float* lo, int64_t n, void* stream);
 PHC_API int phc_gemm_group(const PhcGemmDesc* problems, int32_t count, void* stream);
 PHC_API int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, const float* B, int64_t ldb, int32_t b_kmajor, float* C,
@@ -411,19 +411,18 @@ PHC_API int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, const f
 /* Arithmetic of phc_gemm_tc5s / phc_gemm_group (process-wide switch, read at launch):
  *   PHC_GEMM_FP32_3XTF32      (default) three tensor-core products per fp32 product, fp32-equivalent (the parity path: the
  *                             reference trains with mixed_precision: False);
- *   PHC_GEMM_TF32_SINGLE_PASS one tcgen05 kind::tf32 product: operands truncated to 10 mantissa bits, fp32 accumulate, ~1e-3
+ *   PHC_GEMM_TF32_SINGLE_PASS one tensor-core tf32 product: operands truncated to 10 mantissa bits, fp32 accumulate, ~1e-3
  *                             relative -- the reduced-precision tensor-core mode BASELINE.json configs[3] asks for (bf16-class: the
  *                             same 8-bit exponent, 3 more mantissa bits than bf16), 3x fewer tensor instructions and no split pass.
  *                             OPT-IN, with its own tolerance (tests/test_gpu_gemm_tc5s.py); nothing in the parity tests uses it. */
 #define PHC_GEMM_FP32_3XTF32 0
 #define PHC_GEMM_TF32_SINGLE_PASS 1
 PHC_API int phc_gemm_set_precision(int32_t mode);
-/* tile configuration switch (tests / tools): 1 = 128 x 128 tile per CTA, 2 = 256 x 128 tile per CTA pair, 0 = default */
+/* CTAs per tile (tests / tools): 0, 1 or 2 are accepted; every tile is computed by one CTA */
 PHC_API int phc_gemm_tc5s_set_ctas(int32_t ctas);
-/* tile shape of the one-CTA kernel (tests / tools): 256 = 128 x 256 x 16 tiles (gemm_tc5w.cu, default; env PHC_TC5_TILE=128 selects the
- * other), 128 = 128 x 128 x 32 tiles (gemm_tc5s.cu), 0 = back to the default.  The CTA-pair configuration always uses gemm_tc5s.cu. */
+/* tile shape (tests / tools): 128 = 128 x 128 x 32 tiles (default), 256 = 128 x 256 x 16 tiles, 0 = back to the default */
 PHC_API int phc_gemm_tc5s_set_tile(int32_t width);
-/* tile order of the one-CTA kernel (tests / tools): 1 = tiles drawn from a global counter (default; env PHC_TC5S_SCHED=static turns it
+/* tile order (tests / tools): 1 = tiles drawn from a global counter (default; env PHC_TC5S_SCHED=static turns it
  * off), 0 = static striding (tile t on CTA t mod grid), -1 = back to the default */
 PHC_API int phc_gemm_tc5s_set_sched(int32_t mode);
 /* Humanoid._action_to_pd_targets (phc/env/tasks/humanoid.py:1711-1713) as pre_physics_step applies it (:1540-1556):
@@ -440,6 +439,7 @@ PHC_API int phc_colsum(const float* X, int64_t ld, int32_t M, int32_t N, float a
 /* the same for up to PHC_GEMM_GROUP_MAX matrices in ONE launch (the bias gradients of all stacks at one layer depth):
  * out[n] += alpha * sum_m X[m, n] (always accumulating: `out` holds zeros or earlier contributions).  X 16-byte aligned, ld a multiple
  * of 4 floats and >= N rounded up to 4 (the 4-padded activation workspaces). */
+/* out[n] += alpha * sum_m X[m, n] for each problem, the row blocks added in a fixed order; the problems' out ranges must not overlap */
 typedef struct PhcColsumDesc { const float* X; int64_t ld; int32_t M, N; float alpha; float* out; } PhcColsumDesc;
 PHC_API int phc_colsum_group(const PhcColsumDesc* problems, int32_t count, void* stream);
 
@@ -458,6 +458,8 @@ PHC_API int phc_rms_apply(const float* x, int64_t ldx, int64_t n, int32_t d, con
 PHC_API int phc_rms_apply_update(const float* x, int64_t ldx, int64_t n, int32_t d, const double* mean_apply, const double* var_apply, float eps,
                          float* y, int64_t ldy, const int64_t* row_idx, double* mean, double* var, double* count, void* workspace,
                          void* stream);
+/* device scratch of phc_rms_update / phc_rms_apply_update: one fp64 (sum, sum of squares) pair per column and row strip, the strips
+ * added in a fixed order, so the statistics do not depend on scheduling */
 PHC_API int64_t phc_rms_workspace_bytes(int32_t d);
 PHC_API int phc_rms_update(const float* x, int64_t ldx, int64_t n, int32_t d, double* mean, double* var, double* count,
                    void* workspace, const int64_t* row_idx /* [n] or NULL, as in phc_rms_apply */, void* stream);

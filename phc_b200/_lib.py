@@ -9,7 +9,7 @@ import ctypes as C
 import os
 
 _HERE = os.path.dirname(os.path.abspath(__file__))
-# PHC_LIB_PATH: experiment builds of the SAME sources (phc_b200.build.build_variant, tools/ab_env.sh); default = the in-tree library
+# PHC_LIB_PATH: experiment builds of the SAME sources (phc_b200.build.build_variant); default = the in-tree library
 LIB_PATH = os.environ.get("PHC_LIB_PATH") or os.path.join(_HERE, "lib", "libphc_b200.so")
 
 PHC_FLAG_UPRIGHT = 1 << 0

@@ -1,4 +1,4 @@
-"""Build libphc_b200.so (hand-written sm_100a CUDA + the C ABI of include/phc_b200.h) in-tree with nvcc.
+"""Build libphc_b200.so (hand-written sm_90a CUDA + the C ABI of include/phc_b200.h) in-tree with nvcc.
 
     python -m phc_b200.build            # incremental (per-file mtime check)
     python -m phc_b200.build --force
@@ -19,7 +19,7 @@ OUT_DIR = os.path.join(HERE, "lib")
 OBJ_DIR = os.path.join(OUT_DIR, "obj")
 LIB_PATH = os.path.join(OUT_DIR, "libphc_b200.so")
 
-ARCH = ["-gencode", "arch=compute_100a,code=sm_100a"]
+ARCH = ["-gencode", "arch=compute_90a,code=sm_90a"]
 COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler", "-fvisibility=hidden",
           "--expt-relaxed-constexpr"]
 # per-file extra flags.  The env-side arithmetic mirrors the reference expression by expression: FMA contraction is off
@@ -27,7 +27,6 @@ COMMON = ["-O3", "-std=c++17", "-lineinfo", "-Xcompiler", "-fPIC", "-Xcompiler",
 # (phc_math.cuh explains which and why; PHC_ENV_FMAD=0 builds the step kernel without any contraction for A/B checks).
 SOURCES = {
     "phc_api.cu": [],
-    "gemm_tc5w.cu": [],
     "env_step.cu": ["-fmad=false"] if os.environ.get("PHC_ENV_FMAD", "1") == "0" else [],
     "env_step_fast.cu": [],
     "env_step_wide.cu": [],
@@ -36,8 +35,7 @@ SOURCES = {
     "motion_load.cu": ["-fmad=false"],
     "ppo_scalars.cu": ["-fmad=false"],
     "gemm.cu": [],
-    "gemm_tc5.cu": [],
-    "gemm_tc5s.cu": [],
+    "gemm_wgmma.cu": [],
     "ppo_update.cu": [],
 }
 
@@ -57,7 +55,7 @@ def _newer(src_files, target) -> bool:
 
 
 def build_variant(name: str, flags, source="env_step.cu") -> str:
-    """Experiment builds (tools/ab_env.sh, tools/gpu_r2_s9.sh): the same library with extra -D flags on ONE source file (or a
+    """Experiment builds: the same library with extra -D flags on ONE source file (or a
     list of them), written to lib/alt_<name>/libphc_b200.so; selected at run time with PHC_LIB_PATH.  Never the default."""
     out_dir = os.path.join(OUT_DIR, f"alt_{name}")
     os.makedirs(out_dir, exist_ok=True)

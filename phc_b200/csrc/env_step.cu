@@ -9,7 +9,7 @@
 // -> HBM-bound (about 250 FLOP per 52-byte body).  Blocks are staged into shared memory with TMA 1-D bulk copies
 // (cp.async.bulk + mbarrier: no register staging, one elected lane issues), de-interleaved from shared memory with
 // stride-13 reads (conflict free), results are staged as one observation row in shared memory and leave with
-// coalesced 8-byte stores.  28 envs are resident per SM at J = 24 so N = 4096 is a single wave on 148 SMs.
+// coalesced 8-byte stores.  28 envs are resident per SM at J = 24 so N = 4096 fills 147 SMs (a little over one wave on an H100's 132).
 #include <cuda_runtime.h>
 #include <math.h>
 #include <stdint.h>
@@ -22,11 +22,11 @@
 
 namespace phc {
 
-#ifndef PHC_EXP_WARPS            // experiment knob (tools/ab_env.sh): warps (= envs) per CTA
+#ifndef PHC_EXP_WARPS            // experiment knob (phc_b200.build.build_variant): warps (= envs) per CTA
 #define PHC_EXP_WARPS 4
 #endif
 constexpr int kWarpsPerCta = PHC_EXP_WARPS;
-constexpr int kMinCtasPerSm = 28 / PHC_EXP_WARPS;   // 28 envs resident per SM: 4096 envs = one wave on 148 SMs
+constexpr int kMinCtasPerSm = 28 / PHC_EXP_WARPS;   // 28 envs resident per SM: 4096 envs fill 147 SMs
 struct StepLayout {      // per-warp shared-memory carve-up, in floats (all multiples of 4 -> 16-byte aligned)
   int rslots;            // 2 frame slots of the reward bracket            | the observation row (T == 1) is
   int state;             // J*13 rounded up: the env's simulator block     | staged over these two regions once
@@ -65,7 +65,7 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
   // the warp index through a shuffle: the compiler then KNOWS it (and the env index, and every pointer derived from it) is
   // warp-uniform, keeps them in uniform registers and issues the bulk copies straight from there instead of wrapping each
   // one in a vote + R2UR.BROADCAST loop
-#ifdef PHC_EXP_NO_UNIFORM_WARP      // A/B build (tools/ab_env.sh): the round-1 form
+#ifdef PHC_EXP_NO_UNIFORM_WARP      // A/B build (phc_b200.build.build_variant): the round-1 form
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
 #else
   const int warp = __shfl_sync(0xffffffffu, (int)(threadIdx.x >> 5), 0), lane = threadIdx.x & 31;

@@ -1,6 +1,6 @@
 // Fused env step, steady state of the shipped SMPL configuration, with the phases ordered by INPUT ARRIVAL.
 //
-// What the per-warp timeline of env_step_kernel<1, 24, false, true> showed (tools/timeline_env.py, profiles/env_step_r2_timeline.md):
+// What the per-warp timeline of env_step_kernel<1, 24, false, true> showed (tools/timeline_env.py):
 // at 4096 envs the launch is one wave; every warp asks for its simulator block, its cached reference pose and its dof rows at
 // t = 0 (13.7 MB in flight), its few scalars queue behind them, and -- a warp issues in order -- nothing computed until the first
 // USE of those scalars (the frame bracket, in front of everything else) was satisfied, 2-5 us after entry.  This kernel is the same
@@ -16,9 +16,11 @@
 // complete (AMP slot + the first 356 floats of the observation row after phase 1).  The observation row is staged in two pieces
 // because its head must not overwrite inputs that are still unread: floats [0, 356) in their own region, floats [356, 936) over
 // the consumed [simulator block | cached pose] (356 * 4 bytes is the last 16-byte boundary below the self / task seam at 358).
-// Measured (same box, L2 flushed, PDL launch): 12.3 -> 10.8 us at 4096 envs, 39.5 -> 36.9 us at 16384.
-// One warp per env, lane = body, 4 warps per CTA, 7 CTAs per SM (28 envs per SM: 4096 envs are one wave on 148 SMs).
-// A/B knobs kept for tools/gpu_r2_s19.sh / s20.sh (both measured WORSE, profiles/env_step_r2_*.log): PHC_EXP_CACHE_LATE requests
+// One warp per env, lane = body, 4 warps per CTA, 7 CTAs per SM (28 envs per SM).  On an H100: 7 x 128 threads x 64
+// registers = 57 344 of 65 536, 7 x (31 168 B of shared memory at amp_dim 196 + 1 KB reserved) = 225 344 of 233 472 B, so an eighth CTA
+// does not fit; 132 SMs hold 3 696 envs, and 4096 envs are one full wave plus a 400-env tail on 15 SMs (its cost is not measured
+// separately: it is inside the kernel time bench.py reports).
+// A/B knobs (compile-time, off by default): PHC_EXP_CACHE_LATE requests
 // the cached pose together with the bracket, PHC_EXP_SCALARS_FIRST puts the scalar requests ahead of the simulator block.
 // Launch conditions: exactly those of the FAST instantiation (phc_env_step checks them); reference functions replaced: as
 // env_step.cu (include/phc_b200.h, PhcStepArgs).

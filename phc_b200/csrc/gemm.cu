@@ -12,7 +12,7 @@
 // Precision: fp32-equivalent on the TF32 tensor cores by the 3xTF32 split (a = a_hi + a_lo in registers,
 // acc += a_lo*b_hi + a_hi*b_lo + a_hi*b_hi, fp32 accumulate), because the reference trains in fp32 and the parity
 // bar is 1e-5; a single TF32/BF16 pass (1e-3) would not meet it.  v1 of this kernel issues warp-level mma.sync
-// (m16n8k8) from a cp.async multi-stage pipeline; DESIGN.md tracks the tcgen05/TMEM version that replaces it.
+// (m16n8k8) from a cp.async multi-stage pipeline; gemm_wgmma.cu is the wgmma version the learner uses by default.
 //
 // Epilogue (all optional, applied in this order): alpha scale, + bias[n], ReLU, * (mask[m,n] > 0) (ReLU backward),
 // then either store or atomically accumulate into C (split-K weight gradients accumulate into a zeroed bucket).
@@ -214,7 +214,8 @@ __global__ void __launch_bounds__(GEMM_THREADS, 2) gemm_3xtf32_kernel(const __gr
       }
 }
 
-// column sums: out[n] (+)= sum_m X[m, n]  (bias gradients).  One block per 32 columns, rows strided over threadIdx.y.
+// column sums: out[n] (+)= sum_m X[m, n]  (bias gradients).  One block per 32 columns, rows strided over threadIdx.y; one block
+// owns a column, so the sum does not depend on scheduling.
 __global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ X, int64_t ld, int M, int N,
                                                       float alpha, float* __restrict__ out, int accumulate) {
   __shared__ float s[32][33];
@@ -229,23 +230,29 @@ __global__ void __launch_bounds__(1024) colsum_kernel(const float* __restrict__ 
 #pragma unroll
     for (int i = 0; i < 32; ++i) t += s[i][threadIdx.x];
     t *= alpha;
-    if (accumulate || gridDim.y > 1) atomicAdd(out + n, t);
-    else out[n] = t;
+    out[n] = accumulate ? out[n] + t : t;
   }
 }
 
 // grouped column sums: up to PHC_GEMM_GROUP_MAX matrices in one launch (the bias gradients of every stack at one layer depth).
 // A block is 8 rows x 32 lanes, each lane owns 4 consecutive columns (one 16-byte load per row): 128 columns x 256 rows per block,
-// 8 independent loads in flight per thread; the 8 row partials meet in shared memory and leave as one atomicAdd per column.
+// 8 independent loads in flight per thread; the 8 row partials meet in shared memory and leave as one partial per column and block.
+// The last block of a column chunk to finish adds the partials of the chunk's row blocks in row order: the result does not depend on
+// which block finishes first.
 struct ColsumGroup {
   const float* X[PHC_GEMM_GROUP_MAX];
   float* out[PHC_GEMM_GROUP_MAX];
   int64_t ld[PHC_GEMM_GROUP_MAX];
   int32_t M[PHC_GEMM_GROUP_MAX], N[PHC_GEMM_GROUP_MAX], block_begin[PHC_GEMM_GROUP_MAX + 1], col_chunks[PHC_GEMM_GROUP_MAX];
+  int32_t rows[PHC_GEMM_GROUP_MAX], row_chunks[PHC_GEMM_GROUP_MAX], chunk_begin[PHC_GEMM_GROUP_MAX];
   float alpha[PHC_GEMM_GROUP_MAX];
   int32_t count;
+  float* part;              // [blocks][128] partial sums
+  unsigned int* tickets;    // [column chunks] blocks of the chunk done so far (zero between launches)
 };
-constexpr int CS_ROWS = 256;
+constexpr int CS_MAX_ROW_CHUNKS = 32, CS_SLOTS = 8, CS_MAX_BLOCKS = 4096, CS_MAX_CHUNKS = 1024;
+__device__ float g_cs_part[CS_SLOTS][CS_MAX_BLOCKS][128];
+__device__ unsigned int g_cs_tickets[CS_SLOTS][CS_MAX_CHUNKS];
 
 __global__ void __launch_bounds__(256) colsum_group_kernel(const __grid_constant__ ColsumGroup G) {
   __shared__ float4 part[8][32];
@@ -260,8 +267,8 @@ __global__ void __launch_bounds__(256) colsum_group_kernel(const __grid_constant
   const float* __restrict__ X = G.X[g];
   float4 acc = make_float4(0.f, 0.f, 0.f, 0.f);
   if (c0 < N) {
-    const int r_end = min(M, (rc + 1) * CS_ROWS);
-    int r = rc * CS_ROWS + ry;
+    const int r_end = min(M, (rc + 1) * G.rows[g]);
+    int r = rc * G.rows[g] + ry;
     for (; r + 56 < r_end; r += 64) {
       float4 v[8];
 #pragma unroll
@@ -276,14 +283,30 @@ __global__ void __launch_bounds__(256) colsum_group_kernel(const __grid_constant
   }
   part[ry][lane] = acc;
   __syncthreads();
+  __shared__ bool last;
   if (threadIdx.x < 128) {
+    const float* p = reinterpret_cast<const float*>(&part[0][0]) + threadIdx.x;
+    float t = 0.f;
+#pragma unroll
+    for (int i = 0; i < 8; ++i) t += p[i * 128];
+    G.part[(int64_t)blockIdx.x * 128 + threadIdx.x] = t;
+    __threadfence();
+  }
+  __syncthreads();
+  unsigned int* ticket = G.tickets + G.chunk_begin[g] + cc;
+  if (threadIdx.x == 0) {
+    last = atomicAdd(ticket, 1u) == (unsigned)(G.row_chunks[g] - 1);
+    if (last) *ticket = 0u;                                   // back to zero for the next launch
+  }
+  __syncthreads();
+  if (last && threadIdx.x < 128) {
+    __threadfence();
     const int c = cc * 128 + threadIdx.x;
     if (c < N) {
-      const float* p = reinterpret_cast<const float*>(&part[0][0]) + threadIdx.x;
       float t = 0.f;
-#pragma unroll
-      for (int i = 0; i < 8; ++i) t += p[i * 128];
-      atomicAdd(G.out[g] + c, t * G.alpha[g]);
+      for (int i = 0; i < G.row_chunks[g]; ++i)
+        t += __ldcg(G.part + ((int64_t)G.block_begin[g] + (int64_t)i * G.col_chunks[g] + cc) * 128 + threadIdx.x) * G.alpha[g];
+      G.out[g][c] += t;
     }
   }
 }
@@ -293,7 +316,7 @@ __global__ void __launch_bounds__(256) colsum_group_kernel(const __grid_constant
 extern "C" int phc_colsum_group(const PhcColsumDesc* d, int32_t count, void* stream) {
   if (!d || count < 1 || count > PHC_GEMM_GROUP_MAX) { phc_set_error("phc_colsum_group: 1 <= count <= PHC_GEMM_GROUP_MAX problems"); return PHC_ERR_INVALID_ARG; }
   phc::ColsumGroup G;
-  int n = 0, blocks = 0;
+  int n = 0, blocks = 0, chunks = 0;
   for (int i = 0; i < count; ++i) {
     const PhcColsumDesc& q = d[i];
     if (!q.X || !q.out || q.M < 0 || q.N < 0) { phc_set_error("phc_colsum_group: bad problem (NULL pointer or negative size)"); return PHC_ERR_INVALID_ARG; }
@@ -302,13 +325,37 @@ extern "C" int phc_colsum_group(const PhcColsumDesc* d, int32_t count, void* str
       return PHC_ERR_INVALID_ARG;
     }
     if (q.M == 0 || q.N == 0) continue;
+    for (int j = 0; j < n; ++j)                                 // the last block of a chunk adds without atomics: one writer per column
+      if (q.out < G.out[j] + G.N[j] && G.out[j] < q.out + q.N) { phc_set_error("phc_colsum_group: the problems' out ranges overlap"); return PHC_ERR_INVALID_ARG; }
     G.X[n] = q.X; G.out[n] = q.out; G.ld[n] = q.ld; G.M[n] = q.M; G.N[n] = q.N; G.alpha[n] = q.alpha;
     G.col_chunks[n] = (q.N + 127) / 128;
+    int rows = (q.M + phc::CS_MAX_ROW_CHUNKS - 1) / phc::CS_MAX_ROW_CHUNKS;
+    rows = rows < 256 ? 256 : (rows + 63) / 64 * 64;
+    G.rows[n] = rows;
+    G.row_chunks[n] = (q.M + rows - 1) / rows;
+    G.chunk_begin[n] = chunks;
+    chunks += G.col_chunks[n];
     G.block_begin[n] = blocks;
-    blocks += G.col_chunks[n] * ((q.M + phc::CS_ROWS - 1) / phc::CS_ROWS);
+    blocks += G.col_chunks[n] * G.row_chunks[n];
     ++n;
   }
   if (n == 0) return PHC_OK;
+  if (blocks > phc::CS_MAX_BLOCKS || chunks > phc::CS_MAX_CHUNKS) { phc_set_error("phc_colsum_group: problems too large for one launch"); return PHC_ERR_UNSUPPORTED; }
+  static float* part_base = nullptr;
+  static unsigned int* ticket_base = nullptr;
+  static unsigned int launch_no = 0;
+  if (!part_base) {
+    void* p = nullptr;
+    cudaError_t e = cudaGetSymbolAddress(&p, phc::g_cs_part);
+    if (e != cudaSuccess) return phc_check_cuda(e, "cudaGetSymbolAddress(g_cs_part)");
+    part_base = static_cast<float*>(p);
+    e = cudaGetSymbolAddress(&p, phc::g_cs_tickets);
+    if (e != cudaSuccess) return phc_check_cuda(e, "cudaGetSymbolAddress(g_cs_tickets)");
+    ticket_base = static_cast<unsigned int*>(p);
+  }
+  const unsigned int slot = launch_no++ % phc::CS_SLOTS;      // launches in flight on different streams use different slots
+  G.part = part_base + (size_t)slot * phc::CS_MAX_BLOCKS * 128;
+  G.tickets = ticket_base + (size_t)slot * phc::CS_MAX_CHUNKS;
   G.block_begin[n] = blocks; G.count = n;
   phc::colsum_group_kernel<<<(unsigned)blocks, 256, 0, static_cast<cudaStream_t>(stream)>>>(G); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "colsum_group_kernel launch");
@@ -363,9 +410,7 @@ extern "C" int phc_colsum(const float* X, int64_t ld, int32_t M, int32_t N, floa
                           void* stream) {
   if (!X || !out || M < 0 || N < 0) { phc_set_error("phc_colsum: bad arguments"); return PHC_ERR_INVALID_ARG; }
   if (N == 0) return PHC_OK;
-  int gy = (M + 1023) / 1024; if (gy < 1) gy = 1; if (gy > 64) gy = 64;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  if (gy > 1 && !accumulate) cudaMemsetAsync(out, 0, (size_t)N * 4, st);
-  phc::colsum_kernel<<<dim3((N + 31) / 32, gy), dim3(32, 32), 0, st>>>(X, ld, M, N, alpha, out, accumulate); phc_count_launches(1);
+  phc::colsum_kernel<<<dim3((N + 31) / 32, 1), dim3(32, 32), 0, st>>>(X, ld, M, N, alpha, out, accumulate); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "colsum_kernel launch");
 }

@@ -285,7 +285,7 @@ extern "C" int phc_motion_pack_dofs(const float* dof_pos, const float* dof_vel, 
   if (!dof_pos || !dof_vel || !fj || F < 0 || D < 1 || (reinterpret_cast<uintptr_t>(fj) & 15)) { phc_set_error("phc_motion_pack_dofs: bad arguments"); return PHC_ERR_INVALID_ARG; }
   if (F == 0) return PHC_OK;
   const int JS = phc_motion_dof_stride(D);
-  int64_t g = (F * JS + 255) / 256; if (g > 148 * 16) g = 148 * 16;
+  int64_t g = (F * JS + 255) / 256; if (g > 132 * 16) g = 132 * 16;
   phc::motion_pack_dofs_kernel<<<(unsigned)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(dof_pos, dof_vel, F, D, JS, fj); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "motion_pack_dofs_kernel launch");
 }
@@ -301,7 +301,7 @@ extern "C" int phc_motion_pack(const float* gts, const float* grs, const float* 
   const bool joint = fj && lrs && dvs;
   const int64_t total = F * J;
   const int block = 256;
-  const int grid = (int)((total + block - 1) / block < 148 * 16 ? (total + block - 1) / block : 148 * 16);
+  const int grid = (int)((total + block - 1) / block < 132 * 16 ? (total + block - 1) / block : 132 * 16);
   phc::motion_pack_kernel<<<grid, block, 0, static_cast<cudaStream_t>(stream)>>>(
       gts, grs, gvs, gavs, lrs, dvs, F, J, phc_motion_body_stride(J), phc_motion_joint_stride(J), fb, joint ? fj : nullptr); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "motion_pack_kernel launch");
@@ -424,7 +424,7 @@ extern "C" int phc_amp_window_export_ring(const float* ring, int64_t ring_stride
   }
   if (n == 0) return PHC_OK;
   if ((reinterpret_cast<uintptr_t>(ring) | reinterpret_cast<uintptr_t>(out)) & 15) { phc_set_error("phc_amp_window_export: buffers must be 16-byte aligned"); return PHC_ERR_INVALID_ARG; }
-  int64_t g = (n * num_steps * amp_dim / 4 + 255) / 256; if (g > 148 * 16) g = 148 * 16; if (g < 1) g = 1;
+  int64_t g = (n * num_steps * amp_dim / 4 + 255) / 256; if (g > 132 * 16) g = 132 * 16; if (g < 1) g = 1;
   phc::amp_window_export_kernel<<<(unsigned)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(ring, ring_stride, n, num_steps, amp_dim, head, head_dev, out, out_stride); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "amp_window_export_kernel launch");
 }

@@ -25,4 +25,4 @@ extern "C" void phc_launch_count_add(int64_t n) { if (n > 0) __atomic_fetch_add(
 extern "C" int64_t phc_launch_count(void) { return (int64_t)__atomic_load_n(&g_launches, __ATOMIC_RELAXED); }
 extern "C" const char* phc_last_error(void) { return g_err; }
 extern "C" int phc_version(void) { return 200; }   /* 0.2.0 */
-extern "C" int phc_compiled_sm(void) { return 100; }
+extern "C" int phc_compiled_sm(void) { return 90; }

@@ -127,7 +127,7 @@ adv_apply_kernel(float* __restrict__ adv, int64_t n, const double* __restrict__ 
 static inline int adv_grid(int64_t n) {
   int64_t g = (n + kAdvBlock * 4 - 1) / (kAdvBlock * 4);
   if (g < 1) g = 1;
-  if (g > 148 * 2) g = 148 * 2;
+  if (g > 132 * 2) g = 132 * 2;
   return (int)g;
 }
 

@@ -52,7 +52,8 @@ __global__ void rms_apply_kernel(const float* __restrict__ x, int64_t ldx, int64
   }
 }
 
-// column moments in fp64: acc[0:d] += sum, acc[d:2d] += sum of squares   (acc zeroed by the caller)
+// column moments in fp64 of the block's row strip: acc[y][0:d] = sum, acc[y][d:2d] = sum of squares, y = blockIdx.y (rms_merge_kernel
+// adds the row strips in order, so the moments do not depend on scheduling)
 __global__ void __launch_bounds__(1024) rms_moments_kernel(const float* __restrict__ x, int64_t ldx, int64_t n, int d,
                                                            double* __restrict__ acc, const int64_t* __restrict__ row_idx) {
   __shared__ double s1[32][33], s2[32][33];
@@ -70,8 +71,8 @@ __global__ void __launch_bounds__(1024) rms_moments_kernel(const float* __restri
   if (threadIdx.y == 0 && c < d) {
     double ta = 0.0, tb = 0.0;
     for (int i = 0; i < 32; ++i) { ta += s1[i][threadIdx.x]; tb += s2[i][threadIdx.x]; }
-    atomicAdd(acc + c, ta);
-    atomicAdd(acc + d + c, tb);
+    acc[(int64_t)blockIdx.y * 2 * d + c] = ta;
+    acc[(int64_t)blockIdx.y * 2 * d + d + c] = tb;
   }
 }
 
@@ -116,16 +117,16 @@ __global__ void __launch_bounds__(1024) rms_apply_moments_kernel(const float* __
   if (threadIdx.y == 0 && c < d) {
     double ta = 0.0, tb = 0.0;
     for (int i = 0; i < 32; ++i) { ta += s1[i][threadIdx.x]; tb += s2[i][threadIdx.x]; }
-    atomicAdd(acc + c, ta);
-    atomicAdd(acc + d + c, tb);
+    acc[(int64_t)blockIdx.y * 2 * d + c] = ta;
+    acc[(int64_t)blockIdx.y * 2 * d + d + c] = tb;
   }
 }
 
 // The same two jobs (normalise; normalise + column moments) with V-wide rows per lane: V = 4 (2) consecutive columns per thread as one
 // 16 (8) byte load / store when the row pitches allow it, 4 gathered rows in flight per thread.  Block = 8 warps x 32 lanes: 32 V columns,
-// rows w, w + 8, ... of the block's row strip; the fp64 partial sums of the 8 warps meet in shared memory and leave as one atomicAdd per
+// rows w, w + 8, ... of the block's row strip; the fp64 partial sums of the 8 warps meet in shared memory and leave as one partial per
 // column and block.  Arithmetic per element is that of rms_apply_kernel ((x - mean) / sqrt(var + eps), clamp): results are bit-identical,
-// the moments differ from rms_moments_kernel only in the order of the fp64 additions.
+// the moments differ from rms_moments_kernel only in the order of the fp64 additions (a fixed order in both).
 // (The scalar kernels above: 0.7 TB/s on the gathered 4096 x 1960 AMP rows, 47 us; this one is bound by the gather.)
 template <int V> struct RmsVec;
 template <> struct RmsVec<4> { using T = float4; };
@@ -208,15 +209,16 @@ __global__ void __launch_bounds__(256) rms_apply_vec_kernel(const float* __restr
       if (c < d) {
         double ta = 0.0, tb = 0.0;
         for (int i = 0; i < 8; ++i) { ta += s1[i][threadIdx.x]; tb += s2[i][threadIdx.x]; }
-        atomicAdd(acc + c, ta);
-        atomicAdd(acc + d + c, tb);
+        acc[(int64_t)blockIdx.y * 2 * d + c] = ta;
+        acc[(int64_t)blockIdx.y * 2 * d + d + c] = tb;
       }
     }
   }
 }
 
 // parallel-variance merge of the batch moments into the fp64 running stats (running_mean_std.py:56-68, :99-107)
-__global__ void __launch_bounds__(1024) rms_merge_kernel(const double* __restrict__ acc, int64_t n, int d,
+// (batch moments = the row-strip partials acc[0 .. strips - 1] added in order)
+__global__ void __launch_bounds__(1024) rms_merge_kernel(const double* __restrict__ acc, int strips, int64_t n, int d,
                                                          double* __restrict__ mean, double* __restrict__ var,
                                                          double* __restrict__ count) {
   const double cnt = *count;
@@ -224,8 +226,10 @@ __global__ void __launch_bounds__(1024) rms_merge_kernel(const double* __restric
   const double tot = cnt + bc;
   __syncthreads();
   for (int c = threadIdx.x; c < d; c += blockDim.x) {
-    const double bm = acc[c] / bc;
-    double bv = (acc[d + c] - acc[c] * bm) / (bc - 1.0);       // unbiased, torch.var default
+    double s = 0.0, q = 0.0;
+    for (int y = 0; y < strips; ++y) { s += acc[(int64_t)y * 2 * d + c]; q += acc[(int64_t)y * 2 * d + d + c]; }
+    const double bm = s / bc;
+    double bv = (q - s * bm) / (bc - 1.0);       // unbiased, torch.var default
     if (bv < 0.0) bv = 0.0;
     const double delta = bm - mean[c];
     const double new_mean = mean[c] + delta * bc / tot;
@@ -433,14 +437,28 @@ __global__ void axpy2d_kernel(const float* __restrict__ x, int64_t ldx, float* _
 // ---------------------------------------------------------------------------------------------------------
 // global-norm clip + Adam on the flat parameter bucket
 // ---------------------------------------------------------------------------------------------------------
-__global__ void sumsq_kernel(const float* __restrict__ g, int64_t n, double* __restrict__ out) {
+// sum of squares in fp64: one partial per block (warps added in order), then sum_parts_kernel adds the blocks in order -- the norm
+// that scales the clip does not depend on scheduling
+__global__ void __launch_bounds__(256) sumsq_kernel(const float* __restrict__ g, int64_t n, double* __restrict__ part) {
+  __shared__ double w[8];
   double s = 0.0;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const double v = (double)g[i];
     s += v * v;
   }
   s = wsumd(s);
-  if ((threadIdx.x & 31) == 0) atomicAdd(out, s);
+  if ((threadIdx.x & 31) == 0) w[threadIdx.x >> 5] = s;
+  __syncthreads();
+  if (threadIdx.x == 0) {
+    double t = 0.0;
+    for (int i = 0; i < 8; ++i) t += w[i];
+    part[blockIdx.x] = t;
+  }
+}
+__global__ void sum_parts_kernel(const double* __restrict__ part, int parts, double* __restrict__ out) {
+  double t = 0.0;
+  for (int i = 0; i < parts; ++i) t += part[i];
+  *out = t;
 }
 
 // torch.nn.utils.clip_grad_norm_(max_norm) + torch.optim.Adam(lr, betas, eps, weight_decay=0) in one pass.
@@ -526,9 +544,13 @@ __global__ void act_backward_kernel(float* __restrict__ dy, int64_t ldd, const f
   }
 }
 
+constexpr int RMS_MAX_STRIPS = 32;      // row strips of the column-moment kernels: one fp64 partial pair per strip in the workspace
+constexpr int SUMSQ_SLOTS = 8, SUMSQ_MAX_PARTS = 132 * 8;
+__device__ double g_sumsq_parts[SUMSQ_SLOTS][SUMSQ_MAX_PARTS];
+
 static inline int ew_grid(int64_t total, int block = 256) {
   int64_t g = (total + block - 1) / block;
-  if (g > 148 * 8) g = 148 * 8;
+  if (g > 132 * 8) g = 132 * 8;
   if (g < 1) g = 1;
   return (int)g;
 }
@@ -547,7 +569,7 @@ static int rms_vec_width(const float* x, int64_t ldx, const float* y, int64_t ld
 }
 // rows per block so that the grid is a few waves of 256-thread blocks (multiple of 32 rows: 4 rows in flight x 8 warps)
 static int rms_rows_per_block(int64_t n, int col_blocks) {
-  int64_t want = (int64_t)148 * 8 / (col_blocks > 0 ? col_blocks : 1);
+  int64_t want = (int64_t)132 * 8 / (col_blocks > 0 ? col_blocks : 1);
   if (want < 1) want = 1;
   int64_t rows = (n + want - 1) / want;
   rows = (rows + 31) / 32 * 32;
@@ -572,16 +594,15 @@ extern "C" int phc_rms_apply(const float* x, int64_t ldx, int64_t n, int32_t d, 
   return phc_check_cuda(cudaGetLastError(), "rms_apply_kernel");
 }
 
-extern "C" int64_t phc_rms_workspace_bytes(int32_t d) { return (int64_t)2 * d * sizeof(double); }
+extern "C" int64_t phc_rms_workspace_bytes(int32_t d) { return (int64_t)RMS_MAX_STRIPS * 2 * d * sizeof(double); }
 
 extern "C" int phc_rms_update(const float* x, int64_t ldx, int64_t n, int32_t d, double* mean, double* var, double* count,
                               void* workspace, const int64_t* row_idx, void* stream) {
   if (!x || !mean || !var || !count || !workspace || n < 2 || d < 1 || ldx < d) { phc_set_error("phc_rms_update: bad arguments (needs n >= 2)"); return PHC_ERR_INVALID_ARG; }
   double* acc = static_cast<double*>(workspace);
-  cudaMemsetAsync(acc, 0, (size_t)2 * d * sizeof(double), ST(stream));
-  int gy = (int)((n + 1023) / 1024); if (gy > 32) gy = 32; if (gy < 1) gy = 1;
+  int gy = (int)((n + 1023) / 1024); if (gy > RMS_MAX_STRIPS) gy = RMS_MAX_STRIPS; if (gy < 1) gy = 1;
   rms_moments_kernel<<<dim3((d + 31) / 32, gy), dim3(32, 32), 0, ST(stream)>>>(x, ldx, n, d, acc, row_idx); phc_count_launches(1);
-  rms_merge_kernel<<<1, 1024, 0, ST(stream)>>>(acc, n, d, mean, var, count); phc_count_launches(1);
+  rms_merge_kernel<<<1, 1024, 0, ST(stream)>>>(acc, gy, n, d, mean, var, count); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "rms_update kernels");
 }
 
@@ -592,19 +613,22 @@ extern "C" int phc_rms_apply_update(const float* x, int64_t ldx, int64_t n, int3
     phc_set_error("phc_rms_apply_update: bad arguments (needs n >= 2)"); return PHC_ERR_INVALID_ARG;
   }
   double* acc = static_cast<double*>(workspace);
-  cudaMemsetAsync(acc, 0, (size_t)2 * d * sizeof(double), ST(stream));
   const int V = rms_vec_width(x, ldx, y, ldy);
+  int gy;
   if (V) {
-    const int cb = (d + 32 * V - 1) / (32 * V), rpb = rms_rows_per_block(n, cb);
-    const dim3 grid(cb, (unsigned)((n + rpb - 1) / rpb));
+    const int cb = (d + 32 * V - 1) / (32 * V);
+    int rpb = rms_rows_per_block(n, cb);
+    if ((n + rpb - 1) / rpb > RMS_MAX_STRIPS) rpb = (int)(((n + RMS_MAX_STRIPS - 1) / RMS_MAX_STRIPS + 31) / 32 * 32);
+    gy = (int)((n + rpb - 1) / rpb);
+    const dim3 grid(cb, (unsigned)gy);
     if (V == 4) rms_apply_vec_kernel<4, true><<<grid, 256, 0, ST(stream)>>>(x, ldx, n, d, mean_apply, var_apply, eps, y, ldy, row_idx, acc, rpb);
     else rms_apply_vec_kernel<2, true><<<grid, 256, 0, ST(stream)>>>(x, ldx, n, d, mean_apply, var_apply, eps, y, ldy, row_idx, acc, rpb);
   } else {
-    int gy = (int)((n + 255) / 256); if (gy > 24) gy = 24; if (gy < 1) gy = 1;
+    gy = (int)((n + 255) / 256); if (gy > 24) gy = 24; if (gy < 1) gy = 1;
     rms_apply_moments_kernel<<<dim3((d + 31) / 32, gy), dim3(32, 32), 0, ST(stream)>>>(x, ldx, n, d, mean_apply, var_apply, eps, y, ldy, row_idx, acc);
   }
   phc_count_launches(1);
-  rms_merge_kernel<<<1, 1024, 0, ST(stream)>>>(acc, n, d, mean, var, count); phc_count_launches(1);
+  rms_merge_kernel<<<1, 1024, 0, ST(stream)>>>(acc, gy, n, d, mean, var, count); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "rms_apply_update kernels");
 }
 
@@ -624,7 +648,7 @@ extern "C" int phc_ppo_actor_grad(const float* mu, int64_t ldmu, const float* lo
     phc_set_error("phc_ppo_actor_grad: bad arguments"); return PHC_ERR_INVALID_ARG;
   }
   if (n == 0) return PHC_OK;
-  ppo_actor_grad_kernel<<<(unsigned)((n + 7) / 8 < 148 * 4 ? (n + 7) / 8 : 148 * 4), 256, 0, ST(stream)>>>(mu, ldmu, logstd, actions, old_neglogp, adv, old_mu, old_sigma, n, A,
+  ppo_actor_grad_kernel<<<(unsigned)((n + 7) / 8 < 132 * 4 ? (n + 7) / 8 : 132 * 4), 256, 0, ST(stream)>>>(mu, ldmu, logstd, actions, old_neglogp, adv, old_mu, old_sigma, n, A,
                                                                          e_clip, bound_coef, inv_batch, dmu, lddmu, stats); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "ppo_actor_grad_kernel");
 }
@@ -639,7 +663,7 @@ extern "C" int phc_ppo_grads_gather(const float* mu, int64_t ldmu, const float* 
     phc_set_error("phc_ppo_grads_gather: bad arguments"); return PHC_ERR_INVALID_ARG;
   }
   if (n == 0) return PHC_OK;
-  ppo_actor_grad_kernel<<<(unsigned)((n + 7) / 8 < 148 * 4 ? (n + 7) / 8 : 148 * 4), 256, 0, ST(stream)>>>(mu, ldmu, logstd, actions, old_neglogp, adv, old_mu, old_sigma, n, A,
+  ppo_actor_grad_kernel<<<(unsigned)((n + 7) / 8 < 132 * 4 ? (n + 7) / 8 : 132 * 4), 256, 0, ST(stream)>>>(mu, ldmu, logstd, actions, old_neglogp, adv, old_mu, old_sigma, n, A,
                                                                          e_clip, bound_coef, inv_batch, dmu, lddmu, stats, row_idx); phc_count_launches(1);
   ppo_critic_grad_kernel<<<ew_grid(n), 256, 0, ST(stream)>>>(v, ldv, ret, n, critic_coef, inv_batch, dv, lddv, stats, row_idx); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "ppo_grads_gather kernels");
@@ -693,9 +717,19 @@ extern "C" int phc_axpy2d(const float* x, int64_t ldx, float* y, int64_t ldy, in
 
 extern "C" int phc_grad_sumsq(const float* g, int64_t n, double* out, void* stream) {
   if (!g || !out || n < 0) { phc_set_error("phc_grad_sumsq: bad arguments"); return PHC_ERR_INVALID_ARG; }
-  cudaMemsetAsync(out, 0, sizeof(double), ST(stream));
-  if (n == 0) return PHC_OK;
-  sumsq_kernel<<<ew_grid(n), 256, 0, ST(stream)>>>(g, n, out); phc_count_launches(1);
+  if (n == 0) { cudaMemsetAsync(out, 0, sizeof(double), ST(stream)); return PHC_OK; }
+  static double* base = nullptr;
+  static unsigned int launch_no = 0;
+  if (!base) {
+    void* p = nullptr;
+    cudaError_t e = cudaGetSymbolAddress(&p, g_sumsq_parts);
+    if (e != cudaSuccess) return phc_check_cuda(e, "cudaGetSymbolAddress(g_sumsq_parts)");
+    base = static_cast<double*>(p);
+  }
+  double* part = base + (size_t)(launch_no++ % SUMSQ_SLOTS) * SUMSQ_MAX_PARTS;     // calls in flight on different streams: different slots
+  const int grid = ew_grid(n);
+  sumsq_kernel<<<grid, 256, 0, ST(stream)>>>(g, n, part);
+  sum_parts_kernel<<<1, 1, 0, ST(stream)>>>(part, grid, out); phc_count_launches(2);
   return phc_check_cuda(cudaGetLastError(), "sumsq_kernel");
 }
 
@@ -730,7 +764,7 @@ extern "C" int phc_pd_targets(const float* actions, int64_t lda, int64_t n, int3
     return PHC_ERR_INVALID_ARG;
   }
   if (n == 0) return PHC_OK;
-  int64_t g = (n * num_dofs + 255) / 256; if (g > 148 * 8) g = 148 * 8;
+  int64_t g = (n * num_dofs + 255) / 256; if (g > 132 * 8) g = 132 * 8;
   phc::pd_targets_kernel<<<(unsigned)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(actions, lda, n, num_dofs, num_actions, dof_of_action, offset, scale,
                                                                                   zero_mask, out, ldo); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "pd_targets_kernel launch");

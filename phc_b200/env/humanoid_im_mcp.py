@@ -2,7 +2,7 @@
 
 The agent's action is a weight vector over `num_prim` frozen primitives; the env normalises its own observation with the
 primitives' running statistics, evaluates every primitive, mixes their PD targets with the weights and then steps as
-HumanoidIm does.  Device work per step: phc_rms_apply -> K x 3 tcgen05 GEMMs -> phc_mcp_combine -> fused env step.
+HumanoidIm does.  Device work per step: phc_rms_apply -> K x 3 tensor-core GEMMs -> phc_mcp_combine -> fused env step.
 """
 from __future__ import annotations
 

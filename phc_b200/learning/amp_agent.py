@@ -85,7 +85,7 @@ class RunningMeanStd:
         self.frozen = False
         self.training = True
         self._lib = _lib.load()
-        self._ws = torch.zeros(2 * size, dtype=torch.float64, device=self.device)
+        self._ws = torch.zeros(self._lib.phc_rms_workspace_bytes(self.size) // 8, dtype=torch.float64, device=self.device)
 
     def train(self):
         self.training = True
@@ -319,7 +319,7 @@ class AMPAgent:
     def _network_spec(net):
         """config['network']: a plain dict (this package, tests) or what rl_games' Runner puts there -- a model object whose builder
         keeps the yaml block (`model.network_builder.params`, rl_games 1.1.4 model_builder.py / network_builder.py).  Returns the dict
-        {name, mlp: {units, activation}, disc: {units, activation}, ...} the B200 networks are built from."""
+        {name, mlp: {units, activation}, disc: {units, activation}, ...} the phc_b200 networks are built from."""
         if isinstance(net, dict):
             return net
         for holder in (net, getattr(net, "network_builder", None), getattr(net, "model", None)):
@@ -508,7 +508,6 @@ class AMPAgent:
             self._rollout_graph = self._rollout_out = None      # the motion tables were re-loaded: the captured launches point at the old ones
             self._rollout_calls = 1
         if self._rollout_graph is not None:
-            self.engine.wlo(self.model.critic.layers[0])        # weights written since the last launch (checkpoint load): re-split first
             self._rollout_graph.replay()
             self._lib.phc_launch_count_add(self._rollout_graph_launches)
             return self._rollout_out
@@ -698,8 +697,6 @@ class AMPAgent:
                                          self.opt_step, st))
             if self.engine.backend == "tc5":
                 net.refresh_split()                    # hi/lo operand copies of the updated weights
-            elif self.engine.backend == "tc5s" and self.engine.presplit and self.engine.precision != "tf32":
-                net.refresh_split_lo()                 # the weights' low TF32 term, once per step instead of once per tile visit
 
     def _minibatch_pipeline(self) -> None:
         """The mini_epochs x num_minibatches updates of an epoch (amp_agent.py:460-483), software-pipelined: the gradient
@@ -727,7 +724,7 @@ class AMPAgent:
             self._optimizer_step(scale)
 
     def _update_sequential(self, ds, idx, B, Bd, A, inv_b, st) -> None:
-        """Forward / losses / backward one network after the other, one launch per GEMM (mma.sync and pre-split tcgen05 back ends)."""
+        """Forward / losses / backward one network after the other, one launch per GEMM (mma.sync and pre-split wgmma back ends)."""
         lib, net, eng, T = self._lib, self.model, self.engine, self.timer
         # ---- actor / critic ----------------------------------------------------------------------------------
         with T("update.preproc_obs"):
@@ -792,7 +789,7 @@ class AMPAgent:
         """The minibatch with the grouped GEMM (phc_gemm_group): actor, critic and discriminator advance layer by layer TOGETHER --
         one persistent launch per layer index forward (3 problems), one per layer index backward (dW and dX of the three networks
         plus the step of the gradient-penalty chain that is ready: up to 8 problems) -- instead of ~30 separate GEMM launches whose
-        tile counts each leave a partial last wave on the 148 SMs.
+        tile counts each leave a partial last wave on the 132 SMs.
         forward (grouped) -> loss_fn() writes d loss / d outputs into the workspaces' `dout` -> backward (grouped, with the
         gradient-penalty chain merged in) -> discriminator regularisers.  x / xa are the normalised, zero-padded inputs."""
         lib, net, eng, T = self._lib, self.model, self.engine, self.timer
@@ -854,13 +851,13 @@ class AMPAgent:
         steps = []
         for li in range(L - 1, 0, -1):
             l = hid[li]
-            steps.append(([eng.gdesc(u[li], True, net.weight(l), False, u[li - 1], Bd, l.in_dim, l.out_dim, b_lo=eng.wlo(l), **mask(li - 1))], None))
+            steps.append(([eng.gdesc(u[li], True, net.weight(l), False, u[li - 1], Bd, l.in_dim, l.out_dim, **mask(li - 1))], None))
         l0 = hid[0]
         c = self._disc_coef * self._disc_grad_penalty
 
         def penalty():
             _lib.check(lib.phc_scale_sumsq(g.data_ptr(), g.stride(0), Bd, l0.in_dim, 2.0 * c / Bd, self._stats[10:].data_ptr(), st))
-        steps.append(([eng.gdesc(u[0], True, net.weight(l0), False, g, Bd, l0.in_dim, l0.out_dim, b_lo=eng.wlo(l0))], penalty))
+        steps.append(([eng.gdesc(u[0], True, net.weight(l0), False, g, Bd, l0.in_dim, l0.out_dim)], penalty))
         for li in range(L):
             l = hid[li]
             src = g if li == 0 else e[li - 1]
@@ -868,7 +865,7 @@ class AMPAgent:
             if li == L - 1:
                 after = lambda: eng.colsum(e[L - 1], Bd, hid[L - 1].out_dim, net.weight(head, True))
             steps.append(([eng.gdesc(u[li], False, src, False, net.weight(l, True), l.out_dim, l.in_dim, Bd, accumulate=True, k_splits=group_splits(Bd)),
-                           eng.gdesc(src, True, net.weight(l), True, e[li], Bd, l.out_dim, l.in_dim, b_lo=eng.wlo(l), **mask(li))], after))
+                           eng.gdesc(src, True, net.weight(l), True, e[li], Bd, l.out_dim, l.in_dim, **mask(li))], after))
         return steps
 
     def _disc_grad_penalty_backward(self, x_demo: torch.Tensor, h_demo, Bd: int) -> None:

@@ -1,7 +1,7 @@
 """Frozen-network loaders used on the env side of the hierarchical configs.
 
 Mirrors phc/learning/network_loader.py:53-73 (`load_pnn`): build the K primitive columns from a PNN checkpoint's
-`a2c_network.pnn.actors.K.*` entries and freeze them.  The primitives run through the same tcgen05 GEMM engine as the
+`a2c_network.pnn.actors.K.*` entries and freeze them.  The primitives run through the same tensor-core GEMM engine as the
 learner (MLPEngine); nothing here falls back to torch matmuls.
 """
 from __future__ import annotations

@@ -109,13 +109,9 @@ class AMPNetwork:
         self.num_floats = off
         self.params = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.grads = torch.zeros(off, dtype=torch.float32, device=self.device)
-        # 3xTF32 operand split of the weights for the tcgen05 GEMM (refreshed after every optimiser step)
+        # 3xTF32 operand split of the weights for the pre-split GEMM back end (refreshed after every optimiser step)
         self.params_hi = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.params_lo = torch.zeros(off, dtype=torch.float32, device=self.device)
-        # tc5s: the low TF32 term of the weights (lo = rna_tf32(W - trunc_tf32(W))), the operand the GEMM's splitter warps would
-        # otherwise recompute on every tile visit; refreshed lazily (torch-side writes bump params._version) and after Adam
-        self.params_lo_trunc = torch.zeros(off, dtype=torch.float32, device=self.device)
-        self._lo_version = -1
         self.sigma = torch.full((action_dim,), float(sigma_init), dtype=torch.float32, device=self.device)
         self._init_default(seed)
 
@@ -129,17 +125,6 @@ class AMPNetwork:
         n = self.num_floats
         _lib.check(_lib.load().phc_split_tf32(self.params.data_ptr(), n, 1, n, self.params_hi.data_ptr(), self.params_lo.data_ptr(),
                                               n, _stream()), "phc_split_tf32")
-
-    def refresh_split_lo(self) -> None:
-        """params_lo_trunc <- split_lo(params) (one streaming pass over the bucket); call after anything that writes `params`
-        behind torch's back (the Adam kernel, a collective)."""
-        _lib.check(_lib.load().phc_split_lo(self.params.data_ptr(), self.params_lo_trunc.data_ptr(), self.num_floats, _stream()), "phc_split_lo")
-        self._lo_version = self.params._version
-
-    def weight_lo(self, l: LinearSpec) -> torch.Tensor:
-        if self._lo_version != self.params._version:
-            self.refresh_split_lo()
-        return self.params_lo_trunc[l.w_off:l.w_off + l.out_dim * l.in_pad].view(l.out_dim, l.in_pad)
 
     def bias(self, l: LinearSpec, grad: bool = False) -> torch.Tensor:
         buf = self.grads if grad else self.params
@@ -198,7 +183,7 @@ class AMPNetwork:
 
 def _splits(tiles: int, K: int) -> int:
     """split-K factor for the weight-gradient GEMMs (M, N are layer widths, K is the batch)."""
-    want = max(1, (4 * 148 + tiles - 1) // tiles)      # ~4 tiles per SM: measured 176 vs 211 us (1024x934, K=16384) against 2 per SM
+    want = max(1, (4 * 132 + tiles - 1) // tiles)      # ~4 tiles per SM
     return int(max(1, min(want, K // 512, 64)))
 
 
@@ -224,21 +209,19 @@ class MLPEngine:
         self.lib = _lib.load()
         self.dev = net.device
         self._ws: Dict[Tuple[str, int], Dict[str, torch.Tensor]] = {}
-        # "tc5s" (default): grouped tcgen05 / TMEM / TMA 3xTF32 with the operand split in shared memory (gemm_tc5s.cu);
-        # "tc5": the round-1 kernel with operands pre-split in global memory (gemm_tc5.cu); "mma": warp-level mma.sync 3xTF32
+        # "tc5s" (default): grouped wgmma 3xTF32 with the operand split in shared memory (gemm_wgmma.cu);
+        # "tc5": the same kernel with operands pre-split in global memory (phc_gemm_tc5); "mma": warp-level mma.sync 3xTF32
         # (gemm.cu).  The latter two stay as cross-check implementations (PHC_GEMM=tc5 | mma)
         self.backend = backend or os.environ.get("PHC_GEMM", "tc5s")
         assert self.backend in ("mma", "tc5", "tc5s")
         if precision == "tf32" and self.backend != "tc5s":
             raise ValueError("precision='tf32' (single tensor-core pass) exists on the tc5s back end only")
         self._companions: Dict[Tuple[int, Tuple[int, ...], Tuple[int, ...]], Tuple[torch.Tensor, torch.Tensor]] = {}
-        # pre-split weight operand (PhcGemmDesc.B_lo): only the -DPHC_TC5S_BLO_IN_STAGE build of the library uses it (measured, not adopted)
-        self.presplit = os.environ.get("PHC_TC5S_PRESPLIT", "0") == "1"
         self.gemm_flops = 0.0          # algorithmic fp32 FLOPs (2 M N K) of every grouped launch so far (bench.py reads it)
         if self.backend == "tc5":
             net.refresh_split()
 
-    # -- operand split bookkeeping for the tcgen05 path --------------------------------------------------------------
+    # -- operand split bookkeeping for the pre-split path --------------------------------------------------------------
     def companions(self, t: torch.Tensor) -> Tuple[torch.Tensor, torch.Tensor]:
         """(hi, lo) buffers that shadow activation tensor `t` (same shape / strides)."""
         key = (t.data_ptr(), tuple(t.shape), tuple(t.stride()))
@@ -299,15 +282,10 @@ class MLPEngine:
             _lib.check(rc, "phc_gemm")
 
     # -- grouped launches (tc5s only): one persistent kernel over the tiles of up to PHC_GEMM_GROUP_MAX independent GEMMs ------
-    def gdesc(self, A, a_k, B, b_k, C, M, N, K, alpha=1.0, bias=None, act=0, aux=None, accumulate=False, k_splits=1, b_lo=None):
-        """b_lo: the pre-split low part of B (same shape / stride), see wlo()."""
+    def gdesc(self, A, a_k, B, b_k, C, M, N, K, alpha=1.0, bias=None, act=0, aux=None, accumulate=False, k_splits=1):
         return _lib.PhcGemmDesc(A.data_ptr(), A.stride(0), 1 if a_k else 0, B.data_ptr(), B.stride(0), 1 if b_k else 0, C.data_ptr(),
                                 C.stride(0), M, N, K, alpha, _ptr(bias), act, _ptr(aux), aux.stride(0) if aux is not None else 0,
-                                1 if accumulate else 0, k_splits, _ptr(b_lo))
-
-    def wlo(self, l: LinearSpec) -> Optional[torch.Tensor]:
-        """The pre-split lo view of layer l's weight for a B operand (None: single-pass mode or PHC_TC5S_PRESPLIT=0)."""
-        return self.net.weight_lo(l) if self.presplit and self.precision != "tf32" else None
+                                1 if accumulate else 0, k_splits, None)
 
     def fwd_desc(self, st: MLPStack, li: int, x: torch.Tensor, ws: Dict[str, torch.Tensor]):
         """Layer li of the forward pass of stack st on batch x / workspace ws (the same epilogues as forward())."""
@@ -322,7 +300,7 @@ class MLPEngine:
             out = ws["out"]
             act = _lib.PHC_ACT_NONE if not st.head_relu else (_lib.PHC_ACT_SILU if silu else (_lib.PHC_ACT_RELU_BITS if "obits" in ws else _lib.PHC_ACT_RELU))
             aux = None if not st.head_relu else (ws["z_out"] if silu else ws.get("obits"))
-        return self.gdesc(inp, True, net.weight(l), True, out, B, l.out_dim, l.in_dim, bias=net.bias(l), act=act, aux=aux, b_lo=self.wlo(l))
+        return self.gdesc(inp, True, net.weight(l), True, out, B, l.out_dim, l.in_dim, bias=net.bias(l), act=act, aux=aux)
 
     def bwd_descs(self, st: MLPStack, li: int, x: torch.Tensor, ws: Dict[str, torch.Tensor], dx: Optional[torch.Tensor] = None):
         """(dW, dX) problems of layer li: dW[out, in] += dY^T X (split-K, reduce-add into the gradient bucket) and
@@ -334,13 +312,13 @@ class MLPEngine:
         dxd = None
         if li > 0:
             if st.activation == "silu":
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_SILU_BWD, aux=ws["z"][li - 1], b_lo=self.wlo(l))
+                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_SILU_BWD, aux=ws["z"][li - 1])
             elif "hbits" in ws:
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_MASK_BITS, aux=ws["hbits"][li - 1], b_lo=self.wlo(l))
+                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_MASK_BITS, aux=ws["hbits"][li - 1])
             else:
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, aux=ws["h"][li - 1], b_lo=self.wlo(l))
+                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, aux=ws["h"][li - 1])
         elif dx is not None:
-            dxd = self.gdesc(dY, True, net.weight(l), False, dx, B, l.in_dim, l.out_dim, b_lo=self.wlo(l))
+            dxd = self.gdesc(dY, True, net.weight(l), False, dx, B, l.in_dim, l.out_dim)
         return dw, dxd
 
     def _set_mode(self) -> None:

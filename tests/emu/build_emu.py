@@ -351,16 +351,14 @@ extern "C" int emu_rms_apply(const float* x, int64_t ldx, int64_t n, int32_t d, 
 }
 extern "C" int emu_rms_update(const float* x, int64_t ldx, int64_t n, int32_t d, double* mean, double* var, double* count, double* acc,
                               const int64_t* row_idx) {
-  for (int i = 0; i < 2 * d; ++i) acc[i] = 0.0;                                     // cudaMemsetAsync of phc_rms_update
   int gy = (int)((n + 1023) / 1024); if (gy > 32) gy = 32; if (gy < 1) gy = 1;
   emu_grid((d + 31) / 32, gy, 32, 32, [&] { phc::rms_moments_kernel(x, ldx, n, d, acc, row_idx); });
-  emu_grid(1, 1, 1024, 1, [&] { phc::rms_merge_kernel(acc, n, d, mean, var, count); });
+  emu_grid(1, 1, 1024, 1, [&] { phc::rms_merge_kernel(acc, gy, n, d, mean, var, count); });
   return 0;
 }
 extern "C" int emu_rms_apply_update_vec(const float* x, int64_t ldx, int64_t n, int32_t d, const double* mean_a, const double* var_a, float eps,
                                        float* y, int64_t ldy, const int64_t* row_idx, double* mean, double* var, double* count, double* acc,
                                        int32_t V, int32_t rows_per_block, int32_t moments) {
-  for (int i = 0; i < 2 * d; ++i) acc[i] = 0.0;
   const int cb = (d + 32 * V - 1) / (32 * V), gy = (int)((n + rows_per_block - 1) / rows_per_block);
   emu_grid(cb, gy, 256, 1, [&] {
     if (V == 4 && moments) phc::rms_apply_vec_kernel<4, true>(x, ldx, n, d, mean_a, var_a, eps, y, ldy, row_idx, acc, rows_per_block);
@@ -368,7 +366,7 @@ extern "C" int emu_rms_apply_update_vec(const float* x, int64_t ldx, int64_t n, 
     else if (moments) phc::rms_apply_vec_kernel<2, true>(x, ldx, n, d, mean_a, var_a, eps, y, ldy, row_idx, acc, rows_per_block);
     else phc::rms_apply_vec_kernel<2, false>(x, ldx, n, d, mean_a, var_a, eps, y, ldy, row_idx, nullptr, rows_per_block);
   });
-  if (moments) emu_grid(1, 1, 1024, 1, [&] { phc::rms_merge_kernel(acc, n, d, mean, var, count); });
+  if (moments) emu_grid(1, 1, 1024, 1, [&] { phc::rms_merge_kernel(acc, gy, n, d, mean, var, count); });
   return 0;
 }
 extern "C" int emu_disc_reward(const float* logit, int64_t ld, const float* task, int64_t n, float scale, float w_task, float w_disc,
@@ -393,8 +391,9 @@ extern "C" int emu_disc_logit_grad(const float* logit, int64_t ld, int64_t n_age
 }
 extern "C" int emu_clip_adam(float* p, const float* g, float* m, float* v, int64_t n, double* sumsq, float grad_scale, float max_norm, float lr,
                              float beta1, float beta2, float eps, int64_t step) {
-  *sumsq = 0.0;
-  emu_grid(2, 1, 256, 1, [&] { phc::sumsq_kernel(g, n, sumsq); });
+  double part[2];
+  emu_grid(2, 1, 256, 1, [&] { phc::sumsq_kernel(g, n, part); });
+  phc::sum_parts_kernel(part, 2, sumsq);
   const double bc1 = 1.0 - pow((double)beta1, (double)step), bc2 = 1.0 - pow((double)beta2, (double)step);      // as phc_adam_step
   emu_grid(2, 1, 256, 1, [&] { phc::adam_clip_kernel(p, g, m, v, n, sumsq, grad_scale, max_norm, lr, beta1, beta2, eps, (float)bc1, (float)sqrt(bc2)); });
   return 0;

@@ -26,6 +26,8 @@ What is executed on the reference side (no restatement involved):
   fut.npz      fut_tracks with 3 future samples (the [B, T, J*24] layout of compute_imitation_observations_v6)
   reset.npz    HumanoidAMP._init_amp_obs_ref, MotionLibBase.sample_time_interval
   g1.npz, smplx.npz   the h1.npz / envstep.npz recipes at the shipped shapes beyond 32 bodies (Unitree G1 38 + 1, SMPL-X 52)
+  replay.npz   ReplayBuffer.store / sample (phc/learning/replay_buffer.py): buffer contents and sampled rows
+  dropin_surface.json  parameter lists of the HumanoidIm / AMPAgent methods the drop-in mirrors must accept
 
   python tests/golden/make_golden.py load getup      # regenerate selected files only
 """
@@ -738,6 +740,53 @@ def gen_load():
     save("load.npz", d)
 
 
+REPLAY_SIZE, REPLAY_WIDTH, REPLAY_STORES, REPLAY_SAMPLES = 50, 7, [8, 8, 8, 20, 13, 50, 3], (5, 17, 30)
+
+
+def gen_replay():
+    """The reference ReplayBuffer fed seeded rows (generator seed 1), its permutations drawn from torch's global generator seeded
+    with 5 at construction: partial fill, wrap-around, a full-size store, samples crossing the permutation refresh."""
+    import importlib.util
+    spec = importlib.util.spec_from_file_location("ref_replay_buffer", os.path.join(ref_shim.REF_ROOT, "phc/learning/replay_buffer.py"))
+    mod = importlib.util.module_from_spec(spec)
+    spec.loader.exec_module(mod)
+    torch.manual_seed(5)
+    ref = mod.ReplayBuffer(REPLAY_SIZE, "cpu")
+    g = torch.Generator().manual_seed(1)
+    d = {}
+    for step, n in enumerate(REPLAY_STORES):
+        ref.store({"amp_obs": torch.randn(n, REPLAY_WIDTH, generator=g)})
+        d[f"data_{step}"] = ref._data_buf["amp_obs"].clone()
+        d[f"count_{step}"] = np.array([ref.get_total_count(), ref.get_buffer_size()])
+        for k in REPLAY_SAMPLES:
+            d[f"sample_{step}_{k}"] = ref.sample(k)["amp_obs"]
+    save("replay.npz", d)
+
+
+DROPIN_METHODS = {
+    "HumanoidIm": ("phc.env.tasks.humanoid_im", ["__init__", "_compute_task_obs", "_compute_reward", "_compute_reset", "resample_motions",
+                                                 "get_task_obs_size", "get_task_obs_size_detail", "post_physics_step"]),
+    "AMPAgent": ("phc.learning.amp_agent", ["__init__", "play_steps", "calc_gradients", "train_epoch", "_calc_amp_rewards", "_combine_rewards",
+                                            "_disc_loss", "get_stats_weights", "set_stats_weights", "_preproc_obs"]),
+}
+
+
+def gen_dropin_surface():
+    """[name, positional, has_default] of every parameter of the reference methods the drop-in mirrors stand in for."""
+    import importlib
+    import inspect
+    import json
+    out = {}
+    for cls_name, (mod, names) in DROPIN_METHODS.items():
+        cls = getattr(importlib.import_module(mod), cls_name)
+        for n in names:
+            ps = inspect.signature(getattr(cls, n)).parameters.values()
+            out[f"{cls_name}.{n}"] = [[p.name, p.kind in (p.POSITIONAL_ONLY, p.POSITIONAL_OR_KEYWORD), p.default is not p.empty] for p in ps]
+    with open(os.path.join(HERE, "dropin_surface.json"), "w") as f:
+        json.dump(out, f, indent=1)
+        f.write("\n")
+
+
 if __name__ == "__main__":
     if len(sys.argv) > 1:
         for name in sys.argv[1:]:
@@ -757,3 +806,5 @@ if __name__ == "__main__":
     gen_smplx()
     gen_getup_smplx()
     gen_vr()
+    gen_replay()
+    gen_dropin_surface()

@@ -19,7 +19,7 @@ from unittest.mock import MagicMock
 REF_ROOT = "/root/reference"
 
 _STUB_ROOTS = (
-    "isaacgym", "rl_games", "smpl_sim", "easydict", "hydra", "omegaconf", "gym", "tensorboardX",
+    "isaacgym", "rl_games", "smpl_sim", "easydict", "hydra", "omegaconf", "gym", "tensorboardX", "joblib",
     "open3d", "lxml", "skimage", "termcolor", "imageio", "matplotlib", "wandb", "ipdb", "mujoco",
     "cv2", "smplx", "torchgeometry", "vtk", "pyvista", "sklearn_extra", "gymnasium", "chumpy",
     "stl", "trimesh", "mujoco_py", "pytorch3d", "numpy_stl", "gdown", "autograd", "numba",

@@ -24,7 +24,7 @@ def test_library_exports_every_declared_symbol():
         assert hasattr(lib, s), f"{s} declared in include/phc_b200.h but not exported"
         assert s in _lib.SIGNATURES, f"{s} has no ctypes signature in phc_b200/_lib.py"
     assert set(_lib.SIGNATURES) == set(syms)
-    assert lib.phc_compiled_sm() == 100
+    assert lib.phc_compiled_sm() == 90
     assert lib.phc_self_obs_dim(24, _lib.PHC_FLAG_ROOT_HEIGHT_OBS) == 358
     assert lib.phc_task_obs_dim(24, 1) == 576
     assert lib.phc_amp_obs_dim(19, 4, _lib.PHC_FLAG_ROOT_HEIGHT_OBS) == 196

@@ -1,7 +1,7 @@
 """The fused env-step KERNEL SOURCE on the CPU: phc_b200/csrc/env_step.cu (kernel + layout helpers, verbatim), phc_math.cuh and
 the reductions of phc_common.cuh are compiled with g++ against a small emulation of the CUDA constructs they use
 (tests/emu/: one warp = 32 threads, barrier-based warp collectives, mbarrier / TMA bulk copy stand-ins) and run on the goldens
-of the UNMODIFIED reference -- the same comparisons tests/test_gpu_env_step.py / test_gpu_getup.py make on the B200, here without
+of the UNMODIFIED reference -- the same comparisons tests/test_gpu_env_step.py / test_gpu_getup.py make on the GPU, here without
 a GPU.  The arguments are assembled by the product's own ops.EnvStepPlan (on host tensors).  Tolerances as on the GPU."""
 import os
 import sys

@@ -1,4 +1,4 @@
-"""The construction path of the reference's entry point, on the B200 classes (VERDICT r1 "make the drop-in real"):
+"""The construction path of the reference's entry point, on the phc_b200 classes (VERDICT r1 "make the drop-in real"):
 
   parse_task.py:60     task = eval(args.task)(cfg=cfg, sim_params=..., physics_engine=..., device_type=..., device_id=..., headless=...)
   run_hydra.py:199-262 rl_games builds the agent from params['config'] (env_name / env_config / num_actors / network builder)

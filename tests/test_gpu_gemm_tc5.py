@@ -1,4 +1,4 @@
-"""GPU parity of the tcgen05/TMEM/TMA GEMM (phc_gemm_tc5, 3xTF32 with pre-split operands) in its three layer forms,
+"""GPU parity of the wgmma GEMM with pre-split operands (phc_gemm_tc5, 3xTF32 with pre-split operands) in its three layer forms,
 against an fp64 product with the fp32-equivalence criterion |err| <= tol * |A||B|^T."""
 import math
 
@@ -15,7 +15,8 @@ DEV = "cuda:0"
 
 @pytest.fixture(params=["persistent", "one_tile_per_cta", "cta_pair", "cta_pair_persistent"], autouse=True)
 def tc5_mode(request, monkeypatch):
-    """The four launch variants of the same kernel family (selected by environment variables read per call)."""
+    """The launch-variant environment variables of earlier builds: the kernel no longer reads them, and setting them must not
+    change a result."""
     monkeypatch.delenv("PHC_TC5_PERSIST", raising=False)
     monkeypatch.delenv("PHC_TC5_PAIR", raising=False)
     monkeypatch.delenv("PHC_TC5_PAIRP", raising=False)

@@ -1,5 +1,5 @@
-"""GPU parity of the grouped tcgen05 GEMM with the 3xTF32 split done in shared memory (phc_gemm_tc5s / phc_gemm_group,
-gemm_tc5s.cu) in its three layer forms and both tile configurations (one CTA: 128 x 128; CTA pair: 256 x 128), against an
+"""GPU parity of the grouped wgmma GEMM with the 3xTF32 split done in shared memory (phc_gemm_tc5s / phc_gemm_group,
+gemm_wgmma.cu) in its three layer forms and both tile shapes (128 x 128 x 32, 128 x 256 x 16), against an
 fp64 product with the fp32-equivalence criterion |err| <= tol * |A||B|^T."""
 import ctypes as C
 import math
@@ -17,7 +17,8 @@ DEV = "cuda:0"
 
 @pytest.fixture(params=[(1, 256), (1, 128), (2, 128)], ids=["wide128x256x16", "cta128x128x32", "pair256x128x32"], autouse=True)
 def ctas(request):
-    """The three tile configurations behind phc_gemm_group: gemm_tc5w.cu (default), gemm_tc5s.cu one-CTA and CTA-pair."""
+    """The tile configurations phc_gemm_group accepts: 128 x 256 x 16 and 128 x 128 x 32 tiles; a request for two CTAs per tile is
+    accepted and runs the one-CTA 128 x 128 tiles."""
     lib = _lib.load()
     n, tile = request.param
     _lib.check(lib.phc_gemm_tc5s_set_ctas(n))
@@ -166,7 +167,7 @@ def test_relu_sign_bits_forward_and_masked_backward():
 
 
 def test_single_pass_tf32_mode_has_its_own_tolerance_and_switches_back():
-    """PHC_GEMM_TF32_SINGLE_PASS (opt-in, BASELINE configs[3]): one tcgen05 product per fp32 product -- operands truncated to tf32,
+    """PHC_GEMM_TF32_SINGLE_PASS (opt-in, BASELINE configs[3]): one tensor-core product per fp32 product -- operands truncated to tf32,
     fp32 accumulation: |err| <= 2.5e-3 |A||B|^T (two truncations of 2^-10 each), all three layer forms; switching back restores the
     fp32-equivalent results bit for bit."""
     lib = _lib.load()
@@ -208,9 +209,9 @@ def _desc(A, a_k, B, b_k, Cm, M, N, K, bias=None, act=0, aux=None, b_lo=None):
 
 
 def test_presplit_weight_operand_is_bit_identical_to_the_in_kernel_split():
-    """PhcGemmDesc.B_lo (phc_split_lo of the weights, loaded by TMA) against the splitter warps' own lo tile: the same numbers go to
-    the tensor core, so the products are equal bit for bit -- K-major B (forward), MN-major B (input gradient), ragged edges, and one
-    grouped launch that mixes problems with and without a pre-split operand."""
+    """phc_split_lo computes exactly the low TF32 term the kernel makes from each staged tile (restated on the host), and a launch
+    that is handed a pre-split PhcGemmDesc.B_lo (accepted, not read) gives bit-identical products -- K-major B (forward), MN-major B
+    (input gradient), ragged edges, and one grouped launch that mixes problems with and without B_lo."""
     lib = _lib.load()
     g = torch.Generator().manual_seed(11)
     cases = []
@@ -247,8 +248,6 @@ def test_dynamic_and_static_tile_order_give_the_same_products(ctas):
     """phc_gemm_tc5s_set_sched: tiles drawn from the global counter (default) vs static striding.  A tile's arithmetic does not depend
     on which CTA computes it, so plain stores are bit-identical; many more tiles than CTAs, tiles of very different length in one
     group, and repeated launches (the counters must be back at zero after every launch)."""
-    if ctas != 1:
-        pytest.skip("the CTA-pair kernel has static striding only")
     lib = _lib.load()
     g = torch.Generator().manual_seed(21)
     probs = []

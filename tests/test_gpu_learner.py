@@ -43,7 +43,7 @@ def test_gemm_forward_form(M, N, K):
     g = torch.Generator().manual_seed(M + N + K)
     A, B, bias = torch.randn(M, K, generator=g), torch.randn(N, K, generator=g) / math.sqrt(K), torch.randn(N, generator=g)
     net = AMPNetwork(8, 2, 8, (4,), (4,), device=DEV)
-    eng = MLPEngine(net, backend="mma")           # the tcgen05 kernel has its own file (test_gpu_gemm_tc5.py)
+    eng = MLPEngine(net, backend="mma")           # the pre-split tensor-core kernel has its own file (test_gpu_gemm_tc5.py)
     Ap, Bp = padded(A), padded(B)
     C = torch.zeros(M, round4(N), device=DEV)
     eng.gemm(Ap, True, Bp, True, C, M, N, K, bias=bias.to(DEV), relu=True)

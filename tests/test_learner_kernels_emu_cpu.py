@@ -82,7 +82,7 @@ def test_running_mean_std_kernels_vs_reference_golden(upd):
     g = load("learn.npz")
     d = 12
     mean, var, cnt = torch.zeros(d, dtype=torch.float64), torch.ones(d, dtype=torch.float64), torch.ones((), dtype=torch.float64)
-    acc = torch.zeros(2 * d, dtype=torch.float64)
+    acc = torch.zeros(32 * 2 * d, dtype=torch.float64)      # phc_rms_workspace_bytes(d): 32 row strips
     for i in range(3):
         x = g[f"rms_x{i}"].float().contiguous()
         y = torch.zeros_like(x)
@@ -122,7 +122,7 @@ def test_vectorised_normalise_and_moments_equal_the_scalar_kernels(upd, V, d, ld
     ys, yv, yv2 = torch.zeros(n, ld), torch.full((n, ld), 9.0), torch.full((n, ld), 9.0)
     upd.emu_rms_apply(x.data_ptr(), ld, n, d, mean_a.data_ptr(), var_a.data_ptr(), 1e-5, 0, ys.data_ptr(), ld, idx.data_ptr())
     st = [(torch.full((d,), 0.3, dtype=torch.float64), torch.full((d,), 1.7, dtype=torch.float64), torch.full((), 50.0, dtype=torch.float64)) for _ in range(2)]
-    acc = torch.zeros(2 * d, dtype=torch.float64)
+    acc = torch.zeros(32 * 2 * d, dtype=torch.float64)      # phc_rms_workspace_bytes(d): 32 row strips
     upd.emu_rms_update(x.data_ptr(), ld, n, d, st[0][0].data_ptr(), st[0][1].data_ptr(), st[0][2].data_ptr(), acc.data_ptr(), idx.data_ptr())
     upd.emu_rms_apply_update_vec(x.data_ptr(), ld, n, d, mean_a.data_ptr(), var_a.data_ptr(), 1e-5, yv.data_ptr(), ld, idx.data_ptr(),
                                  st[1][0].data_ptr(), st[1][1].data_ptr(), st[1][2].data_ptr(), acc.data_ptr(), V, 32, 1)

@@ -1,4 +1,5 @@
-"""Microbenchmark of the MLP GEMM variants on the PPO shapes (diagnostic; numbers for profiles/, not bench values).
+"""Microbenchmark of the MLP GEMM variants on the PPO shapes (diagnostic, not bench values): phc_gemm_tc5 (pre-split operands),
+phc_gemm (mma.sync), phc_gemm_tc5s with 128 x 128 x 32 (s128) and 128 x 256 x 16 (w256) tiles.
 usage: python tools/bench_gemm.py [iters]   -- prints per shape/variant: us, TFLOP/s of tensor work (3 MMAs per product)."""
 import os
 import sys
@@ -33,32 +34,17 @@ def run(name, M, N, K, a_k, b_k, splits=1, mask=False, split_out=False):
     Mk = torch.randn(M, r4(N), device=dev) if mask else None
     Ah, Al = split(A)
     Bh, Bl = split(B)
-    Blo = torch.empty_like(B)
-    _lib.check(lib.phc_split_lo(B.data_ptr(), Blo.data_ptr(), B.numel(), None))
     acc = 1 if splits > 1 else 0
-    variants = [("persist", {}), ("plain", {"PHC_TC5_PERSIST": "0"}), ("pair", {"PHC_TC5_PAIR": "1"}),
-                ("pairp", {"PHC_TC5_PAIRP": "1"}), ("mma.sync", None), ("s1", 1), ("w", 3), ("s1p", "presplit1"), ("s2", 2), ("s2p", "presplit2")]
+    variants = [("presplit", "tc5"), ("mma.sync", None), ("s128", 128), ("w256", 256)]
     out = []
     for vname, env in variants:
         if only and vname not in only.split(","):
             continue
         if isinstance(env, int):
-            lib.phc_gemm_tc5s_set_ctas(1 if env == 3 else env)
-            lib.phc_gemm_tc5s_set_tile(256 if env == 3 else 128)
-        if isinstance(env, str):
-            lib.phc_gemm_tc5s_set_ctas(int(env[-1]))
-            lib.phc_gemm_tc5s_set_tile(128)
-        for k in ("PHC_TC5_PERSIST", "PHC_TC5_PAIR", "PHC_TC5_PAIRP"):
-            os.environ.pop(k, None)
-        if isinstance(env, dict):
-            os.environ.update(env)
+            lib.phc_gemm_tc5s_set_tile(env)
 
         def call():
-            if isinstance(env, str):      # B's lo tile pre-split in global memory (weights), loaded by TMA
-                d = _lib.PhcGemmDesc(A.data_ptr(), A.stride(0), int(a_k), B.data_ptr(), B.stride(0), int(b_k), C.data_ptr(), C.stride(0), M, N, K, 1.0,
-                                     None, 0, None if Mk is None else Mk.data_ptr(), 0 if Mk is None else Mk.stride(0), acc, splits, Blo.data_ptr())
-                return lib.phc_gemm_group((_lib.PhcGemmDesc * 1)(d), 1, None)
-            if isinstance(env, int):      # split in shared memory (gemm_tc5s.cu): raw operands
+            if isinstance(env, int):      # split in shared memory (gemm_wgmma.cu): raw operands
                 return lib.phc_gemm_tc5s(A.data_ptr(), A.stride(0), int(a_k), B.data_ptr(), B.stride(0), int(b_k), C.data_ptr(), C.stride(0),
                                          M, N, K, 1.0, None, 0, None if Mk is None else Mk.data_ptr(), 0 if Mk is None else Mk.stride(0), acc, splits, None)
             if env is None:

@@ -1,5 +1,5 @@
 """Small driver for ncu: runs the fused env-step kernel (4096 envs, one clip per env, L2 flushed between launches),
-one GAE pass and one PPO/AMP minibatch.  Used only to capture profiles/ (never for bench numbers)."""
+one GAE pass and one PPO/AMP minibatch.  Used only for profiler captures (never for bench numbers)."""
 import os
 import sys
 

@@ -1,6 +1,6 @@
 """ncu driver for the MLP GEMMs: one warm launch and one profiled launch of three PPO shapes for ONE kernel variant.
-usage: python tools/profile_gemm.py {persist|plain|s1|s2|w}     (capture with: ncu -k regex:gemm_tc5 -s 3 -c 3 ...)
-s1 / s2: gemm_tc5s.cu one-CTA / CTA-pair (128 x 128 x 32 tiles); w: gemm_tc5w.cu (128 x 256 x 16 tiles)."""
+usage: python tools/profile_gemm.py {presplit|s|w}     (capture with: ncu -k regex:gemm_wgmma -s 3 -c 3 ...)
+presplit: phc_gemm_tc5 (operands pre-split in global memory); s: 128 x 128 x 32 tiles; w: 128 x 256 x 16 tiles."""
 import os
 import sys
 
@@ -11,16 +11,9 @@ from phc_b200 import _lib
 
 lib = _lib.load()
 dev = "cuda:0"
-variant = sys.argv[1] if len(sys.argv) > 1 else "s2"
+variant = sys.argv[1] if len(sys.argv) > 1 else "s"
 r4 = lambda x: (x + 3) & ~3
-if variant == "plain":
-    os.environ["PHC_TC5_PERSIST"] = "0"
-if variant in ("s1", "s2"):
-    lib.phc_gemm_tc5s_set_ctas(int(variant[1]))
-    lib.phc_gemm_tc5s_set_tile(128)
-if variant == "w":
-    lib.phc_gemm_tc5s_set_ctas(1)
-    lib.phc_gemm_tc5s_set_tile(256)
+lib.phc_gemm_tc5s_set_tile(256 if variant == "w" else 128)
 
 
 def split(x):
@@ -36,7 +29,7 @@ def make(M, N, K, a_k, b_k, splits=1, mask=False, bias=False, relu=False):
     Mk = torch.randn(M, r4(N), device=dev) if mask else None
     bs = torch.randn(N, device=dev) if bias else None
     acc = 1 if splits > 1 else 0
-    if variant in ("s1", "s2", "w"):
+    if variant in ("s", "w"):
         return lambda: lib.phc_gemm_tc5s(A.data_ptr(), A.stride(0), int(a_k), B.data_ptr(), B.stride(0), int(b_k), C.data_ptr(), C.stride(0), M, N, K,
                                          1.0, None if bs is None else bs.data_ptr(), int(relu), None if Mk is None else Mk.data_ptr(),
                                          0 if Mk is None else Mk.stride(0), acc, splits, None), (A, B, C, Mk, bs)
