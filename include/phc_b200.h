@@ -387,7 +387,11 @@ PHC_API int phc_gemm_tc5(const float* A_hi, const float* A_lo, int64_t lda, int3
  * copies.  A, B, C 16-byte aligned; lda, ldb, ldc multiples of 4.
  * phc_gemm_group runs up to PHC_GEMM_GROUP_MAX independent problems (e.g. the same layer of actor, critic and
  * discriminator: network_builder.py:105-124 builds three separate nn.Sequential stacks that the reference evaluates one
- * after the other) as ONE persistent launch over the union of their tiles. */
+ * after the other) as ONE persistent launch over the union of their tiles.
+ * Reproducibility: split-K slices add into C in slice order, and problems of one launch that accumulate into the SAME C (same
+ * pointer, M, N and ldc) add one after the other in problem order, each with its slices in order; the result is the same bit for
+ * bit from run to run.  Write hazards are refused (PHC_ERR_INVALID_ARG): the spans [C, C + (M-1)*ldc + N) of two non-empty
+ * problems of one launch must not overlap, except for such a same-C accumulating group. */
 #define PHC_GEMM_GROUP_MAX 8
 typedef struct PhcGemmDesc {
   const float* A; int64_t lda; int32_t a_kmajor;
@@ -469,7 +473,9 @@ PHC_API int phc_gaussian_sample(const float* mu, int64_t ldmu, const float* logs
                         float* actions, float* neglogp, float* mus, float* sigmas, void* stream);
 /* Actor side of AMPAgent.calc_gradients (amp_agent.py:604-641): neglogp of the stored actions, CommonAgent._actor_loss
  * (common_agent.py:564-574), bound_loss (:512-520), policy_kl; writes d(total loss)/d(mu) = inv_batch * (...).
- * stats (float[16], caller-zeroed, sums over rows): [0] actor loss [1] bound loss [2] clipped count [3] kl [4] entropy */
+ * stats (float[16], caller-zeroed, sums over rows): [0] actor loss [1] bound loss [2] clipped count [3] kl [4] entropy
+ * Every `stats` / `stat` sum of the kernels below is added in a fixed order (per-block partials, then the blocks in order), so it
+ * is the same bit for bit from run to run; launches that add into the same statistic must be ordered (one stream). */
 PHC_API int phc_ppo_actor_grad(const float* mu, int64_t ldmu, const float* logstd, const float* actions,
                        const float* old_neglogp, const float* adv, const float* old_mu, const float* old_sigma, int64_t n,
                        int32_t A, float e_clip, float bound_coef, float inv_batch, float* dmu, int64_t lddmu, float* stats,

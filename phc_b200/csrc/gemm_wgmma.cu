@@ -520,6 +520,29 @@ static int validate_group(const PhcGemmDesc* d, int32_t count) {
     if (ks > 1 && (!g.accumulate || g.act || g.aux)) { phc_set_error("phc_gemm_group: split-K needs accumulate=1 and a linear epilogue"); return PHC_ERR_INVALID_ARG; }
     if (g.B_lo && (reinterpret_cast<uintptr_t>(g.B_lo) & 15)) { phc_set_error("phc_gemm_group: B_lo must be 16-byte aligned"); return PHC_ERR_INVALID_ARG; }
   }
+  // write hazards: the C spans [C, C + (M - 1) ldc + N) of two problems may only overlap when both accumulate into the same C with
+  // the same shape -- they then share a turnstile and add in problem order; any other overlap would race (plain stores, or
+  // unordered atomics of accumulating problems with different C)
+  auto span = [](const PhcGemmDesc& g, uintptr_t& lo, uintptr_t& hi) {
+    lo = reinterpret_cast<uintptr_t>(g.C);
+    hi = lo + (uintptr_t)(((int64_t)g.M - 1) * g.ldc + g.N) * sizeof(float);
+  };
+  for (int i = 0; i < count; ++i) {
+    const PhcGemmDesc& a = d[i];
+    if (a.M == 0 || a.N == 0) continue;
+    uintptr_t a0, a1;
+    span(a, a0, a1);
+    for (int j = 0; j < i; ++j) {
+      const PhcGemmDesc& b = d[j];
+      if (b.M == 0 || b.N == 0) continue;
+      uintptr_t b0, b1;
+      span(b, b0, b1);
+      if (a0 >= b1 || b0 >= a1) continue;
+      if (a.accumulate && b.accumulate && a.C == b.C && a.M == b.M && a.N == b.N && a.ldc == b.ldc) continue;
+      phc_set_error("phc_gemm_group: two problems write overlapping C ranges (only accumulating problems on the same C with the same M, N, ldc may)");
+      return PHC_ERR_INVALID_ARG;
+    }
+  }
   return PHC_OK;
 }
 

@@ -30,6 +30,75 @@ __device__ __forceinline__ double wsumd(double v) {
   return v;
 }
 
+// Loss statistics in a fixed order.  Every block leaves its K totals in a library-owned partial buffer; the last block to finish
+// (a ticket, as in colsum_group_kernel) adds the partials of all blocks -- thread t the blocks t, t + blockDim.x, ... in order, then
+// the warps in order -- into out[0 .. K).  The sums do not depend on which block finishes first, so they repeat bit for bit.
+// Launches rotate through STAT_SLOTS partial buffers and tickets (the kernels' `slot` argument), so that launches in flight on
+// different streams never share one.
+constexpr int STAT_SLOTS = 8, STAT_MAX_BLOCKS = 132 * 8, STAT_MAX_K = 5;
+__device__ float g_stat_parts[STAT_SLOTS][STAT_MAX_BLOCKS * STAT_MAX_K];
+__device__ unsigned int g_stat_tickets[STAT_SLOTS];      // blocks of the launch done so far (zero between launches)
+
+// The partials travel between blocks: the writer fences them before it takes the ticket, the last block reads them from L2.  The
+// host compilation of this source (the CPU emulation of the kernels) runs one block at a time and needs neither.
+#if defined(__CUDACC__)
+#define PHC_GRID_FENCE() __threadfence()
+#define PHC_LOAD_L2(p) __ldcg(p)
+#else
+#define PHC_GRID_FENCE() ((void)0)
+#define PHC_LOAD_L2(p) (*(p))
+#endif
+
+// blk[0 .. K): this block's totals in shared memory, complete for every thread; blockDim.x is a multiple of 32, gridDim.x <= STAT_MAX_BLOCKS
+template <int K>
+__device__ void stats_fixed_order(const float* blk, float* __restrict__ out, unsigned int slot) {
+  __shared__ bool last;
+  __shared__ float wpart[32];
+  float* part = g_stat_parts[slot % STAT_SLOTS];
+  unsigned int* ticket = g_stat_tickets + slot % STAT_SLOTS;
+  if (threadIdx.x == 0) {
+    for (int k = 0; k < K; ++k) part[(int64_t)blockIdx.x * K + k] = blk[k];
+    PHC_GRID_FENCE();
+    last = atomicAdd(ticket, 1u) == gridDim.x - 1;
+    if (last) *ticket = 0u;                             // back to zero for the next launch
+  }
+  __syncthreads();
+  if (!last) return;                                    // (block-uniform)
+  PHC_GRID_FENCE();
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+  for (int k = 0; k < K; ++k) {
+    float t = 0.f;
+    for (int b = threadIdx.x; b < (int)gridDim.x; b += blockDim.x) t += PHC_LOAD_L2(part + (int64_t)b * K + k);
+    t = wsum(t);
+    if (lane == 0) wpart[w] = t;
+    __syncthreads();
+    if (threadIdx.x == 0) {
+      float s = 0.f;
+      for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += wpart[i];
+      out[k] += s;
+    }
+    __syncthreads();
+  }
+}
+
+// the block's totals of K per-thread values into blk[0 .. K) (shared memory): shuffles within a warp, then the warps in order
+template <int K>
+__device__ __forceinline__ void block_totals(float (&v)[K], float* blk) {
+  __shared__ float wv[32][K];
+  const int lane = threadIdx.x & 31, w = threadIdx.x >> 5;
+#pragma unroll
+  for (int k = 0; k < K; ++k) v[k] = wsum(v[k]);
+  if (lane == 0)
+    for (int k = 0; k < K; ++k) wv[w][k] = v[k];
+  __syncthreads();
+  if (threadIdx.x < K) {
+    float t = 0.f;
+    for (int i = 0; i < (int)(blockDim.x >> 5); ++i) t += wv[i][threadIdx.x];
+    blk[threadIdx.x] = t;
+  }
+  __syncthreads();
+}
+
 // ---------------------------------------------------------------------------------------------------------
 // RunningMeanStd
 // ---------------------------------------------------------------------------------------------------------
@@ -280,11 +349,11 @@ ppo_actor_grad_kernel(const float* __restrict__ mu, int64_t ldmu, const float* _
                       const float* __restrict__ adv, const float* __restrict__ old_mu,
                       const float* __restrict__ old_sigma, int64_t n, int A, float e_clip, float bound_coef,
                       float inv_batch, float* __restrict__ dmu, int64_t lddmu, float* __restrict__ stats,
-                      const int64_t* __restrict__ row_idx = nullptr) {
+                      const int64_t* __restrict__ row_idx = nullptr, unsigned int slot = 0) {
   // row_idx (optional): the minibatch is INDEX-COMPOSED -- actions / old_neglogp / adv / old_mu / old_sigma are the epoch's dataset
   // arrays and row r of the minibatch is their row row_idx[r] (mu / dmu are in minibatch order); saves six gather passes per minibatch.
   // one warp per row, rows strided over the grid; the five batch statistics are accumulated per warp, folded per block in
-  // shared memory and leave with ONE atomic per block and statistic (per-row atomics on five addresses serialise: 140 us)
+  // shared memory and leave as ONE partial per block and statistic (stats_fixed_order)
   const int lane = threadIdx.x & 31, wib = threadIdx.x >> 5;
   const int64_t warps_total = (int64_t)gridDim.x * (blockDim.x >> 5);
   float st[5] = {0.f, 0.f, 0.f, 0.f, 0.f};
@@ -325,36 +394,40 @@ ppo_actor_grad_kernel(const float* __restrict__ mu, int64_t ldmu, const float* _
     st[3] += kl;
     st[4] += ls + 0.5f * (1.0f + 1.8378770664093453f) * (float)A;          // Normal entropy summed over actions
   }
-  __shared__ float sh[8][5];
+  __shared__ float sh[8][5], blk[5];
   if (lane == 0)
     for (int k = 0; k < 5; ++k) sh[wib][k] = st[k];
   __syncthreads();
   if (threadIdx.x < 5) {
     float t = 0.f;
     for (int w = 0; w < (int)(blockDim.x >> 5); ++w) t += sh[w][threadIdx.x];
-    atomicAdd(stats + threadIdx.x, t);
+    blk[threadIdx.x] = t;
   }
+  __syncthreads();
+  stats_fixed_order<5>(blk, stats, slot);
 }
 
 // critic: c_loss = (ret - v)^2 (clip_value False); dv = coef * 2 (v - ret) / batch.   stats[5] += sum c_loss
 __global__ void ppo_critic_grad_kernel(const float* __restrict__ v, int64_t ldv, const float* __restrict__ ret, int64_t n,
                                        float coef, float inv_batch, float* __restrict__ dv, int64_t lddv,
-                                       float* __restrict__ stats, const int64_t* __restrict__ row_idx = nullptr) {
-  float loss = 0.f;
+                                       float* __restrict__ stats, const int64_t* __restrict__ row_idx = nullptr,
+                                       unsigned int slot = 0) {
+  float loss[1] = {0.f};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float d = v[i * ldv] - ret[row_idx ? row_idx[i] : i];
-    loss += d * d;
+    loss[0] += d * d;
     dv[i * lddv] = coef * 2.0f * d * inv_batch;
   }
-  loss = wsum(loss);
-  if ((threadIdx.x & 31) == 0) atomicAdd(stats + 5, loss);
+  __shared__ float blk[1];
+  block_totals<1>(loss, blk);
+  stats_fixed_order<1>(blk, stats + 5, slot);
 }
 
 // discriminator prediction loss: BCE-with-logits against 0 (agent + replay rows) / 1 (demo rows), 0.5 * (neg + pos)
 // dl = coef * 0.5 * dBCE/dlogit / rows.  stats[6] += sum softplus(x) agent, [7] += sum softplus(-x) demo,
 // [8] += #(agent logit < 0), [9] += #(demo logit > 0)
 __global__ void disc_logit_grad_kernel(const float* __restrict__ logit, int64_t ld, int64_t n_agent, int64_t n_demo,
-                                       float coef, float* __restrict__ dlogit, int64_t ldd, float* __restrict__ stats) {
+                                       float coef, float* __restrict__ dlogit, int64_t ldd, float* __restrict__ stats, unsigned int slot = 0) {
   float la = 0.f, lp = 0.f, ca = 0.f, cd = 0.f;
   const int64_t n = n_agent + n_demo;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
@@ -371,10 +444,10 @@ __global__ void disc_logit_grad_kernel(const float* __restrict__ logit, int64_t 
       dlogit[i * ldd] = coef * 0.5f * (sig - 1.0f) / (float)n_demo;
     }
   }
-  la = wsum(la); lp = wsum(lp); ca = wsum(ca); cd = wsum(cd);
-  if ((threadIdx.x & 31) == 0) {
-    atomicAdd(stats + 6, la); atomicAdd(stats + 7, lp); atomicAdd(stats + 8, ca); atomicAdd(stats + 9, cd);
-  }
+  float v[4] = {la, lp, ca, cd};
+  __shared__ float blk[4];
+  block_totals<4>(v, blk);
+  stats_fixed_order<4>(blk, stats + 6, slot);
 }
 
 // disc reward (amp_agent.py:864-878) fused with _combine_rewards (:848-853):
@@ -401,36 +474,39 @@ __global__ void relu_mask_row_kernel(const float* __restrict__ h, int64_t ldh, c
   }
 }
 
-// x *= alpha in place and stats[slot] += sum(x_before^2)      (gradient penalty: g -> dP/dg, keeps sum ||g||^2)
-__global__ void scale_sumsq_kernel(float* __restrict__ x, int64_t ld, int64_t n, int d, float alpha, float* __restrict__ stat) {
+// x *= alpha in place and *stat += sum(x_before^2)      (gradient penalty: g -> dP/dg, keeps sum ||g||^2)
+__global__ void scale_sumsq_kernel(float* __restrict__ x, int64_t ld, int64_t n, int d, float alpha, float* __restrict__ stat,
+                                   unsigned int slot = 0) {
   const int64_t total = n * d;
-  float s = 0.f;
+  float s[1] = {0.f};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / d;
     const int c = (int)(i - r * d);
     const float v = x[r * ld + c];
-    s += v * v;
+    s[0] += v * v;
     x[r * ld + c] = v * alpha;
   }
-  s = wsum(s);
-  if ((threadIdx.x & 31) == 0) atomicAdd(stat, s);
+  __shared__ float blk[1];
+  block_totals<1>(s, blk);
+  stats_fixed_order<1>(blk, stat, slot);
 }
 
-// y += alpha * x over a strided [rows, cols] block (weight decay / logit regulariser gradients)
+// y += alpha * x over a strided [rows, cols] block (weight decay / logit regulariser gradients); sumsq_stat (optional) += sum(x^2)
 __global__ void axpy2d_kernel(const float* __restrict__ x, int64_t ldx, float* __restrict__ y, int64_t ldy, int64_t rows,
-                              int cols, float alpha, float* __restrict__ sumsq_stat) {
+                              int cols, float alpha, float* __restrict__ sumsq_stat, unsigned int slot = 0) {
   const int64_t total = rows * cols;
-  float s = 0.f;
+  float s[1] = {0.f};
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < total; i += (int64_t)gridDim.x * blockDim.x) {
     const int64_t r = i / cols;
     const int c = (int)(i - r * cols);
     const float v = x[r * ldx + c];
     y[r * ldy + c] += alpha * v;
-    s += v * v;
+    s[0] += v * v;
   }
-  if (sumsq_stat) {
-    s = wsum(s);
-    if ((threadIdx.x & 31) == 0) atomicAdd(sumsq_stat, s);
+  if (sumsq_stat) {                                      // (kernel argument: grid-uniform)
+    __shared__ float blk[1];
+    block_totals<1>(s, blk);
+    stats_fixed_order<1>(blk, sumsq_stat, slot);
   }
 }
 
@@ -577,6 +653,12 @@ static int rms_rows_per_block(int64_t n, int col_blocks) {
   return (int)rows;
 }
 
+// the partial buffer and ticket of the next loss-statistics launch (stats_fixed_order)
+static unsigned int next_stat_slot() {
+  static unsigned int launch_no = 0;
+  return launch_no++ % STAT_SLOTS;
+}
+
 extern "C" int phc_rms_apply(const float* x, int64_t ldx, int64_t n, int32_t d, const double* mean, const double* var,
                              float eps, int32_t unnorm, float* y, int64_t ldy, const int64_t* row_idx, void* stream) {
   if (!x || !mean || !var || !y || n < 0 || d < 1 || ldx < d || ldy < d) { phc_set_error("phc_rms_apply: bad arguments"); return PHC_ERR_INVALID_ARG; }
@@ -649,7 +731,7 @@ extern "C" int phc_ppo_actor_grad(const float* mu, int64_t ldmu, const float* lo
   }
   if (n == 0) return PHC_OK;
   ppo_actor_grad_kernel<<<(unsigned)((n + 7) / 8 < 132 * 4 ? (n + 7) / 8 : 132 * 4), 256, 0, ST(stream)>>>(mu, ldmu, logstd, actions, old_neglogp, adv, old_mu, old_sigma, n, A,
-                                                                         e_clip, bound_coef, inv_batch, dmu, lddmu, stats); phc_count_launches(1);
+                                                                         e_clip, bound_coef, inv_batch, dmu, lddmu, stats, nullptr, next_stat_slot()); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "ppo_actor_grad_kernel");
 }
 
@@ -664,8 +746,8 @@ extern "C" int phc_ppo_grads_gather(const float* mu, int64_t ldmu, const float* 
   }
   if (n == 0) return PHC_OK;
   ppo_actor_grad_kernel<<<(unsigned)((n + 7) / 8 < 132 * 4 ? (n + 7) / 8 : 132 * 4), 256, 0, ST(stream)>>>(mu, ldmu, logstd, actions, old_neglogp, adv, old_mu, old_sigma, n, A,
-                                                                         e_clip, bound_coef, inv_batch, dmu, lddmu, stats, row_idx); phc_count_launches(1);
-  ppo_critic_grad_kernel<<<ew_grid(n), 256, 0, ST(stream)>>>(v, ldv, ret, n, critic_coef, inv_batch, dv, lddv, stats, row_idx); phc_count_launches(1);
+                                                                         e_clip, bound_coef, inv_batch, dmu, lddmu, stats, row_idx, next_stat_slot()); phc_count_launches(1);
+  ppo_critic_grad_kernel<<<ew_grid(n), 256, 0, ST(stream)>>>(v, ldv, ret, n, critic_coef, inv_batch, dv, lddv, stats, row_idx, next_stat_slot()); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "ppo_grads_gather kernels");
 }
 
@@ -673,14 +755,14 @@ extern "C" int phc_ppo_critic_grad(const float* v, int64_t ldv, const float* ret
                                    float* dv, int64_t lddv, float* stats, void* stream) {
   if (!v || !ret || !dv || !stats || n < 0 || ldv < 1 || lddv < 1) { phc_set_error("phc_ppo_critic_grad: bad arguments"); return PHC_ERR_INVALID_ARG; }
   if (n == 0) return PHC_OK;
-  ppo_critic_grad_kernel<<<ew_grid(n), 256, 0, ST(stream)>>>(v, ldv, ret, n, coef, inv_batch, dv, lddv, stats); phc_count_launches(1);
+  ppo_critic_grad_kernel<<<ew_grid(n), 256, 0, ST(stream)>>>(v, ldv, ret, n, coef, inv_batch, dv, lddv, stats, nullptr, next_stat_slot()); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "ppo_critic_grad_kernel");
 }
 
 extern "C" int phc_disc_logit_grad(const float* logit, int64_t ld, int64_t n_agent, int64_t n_demo, float coef,
                                    float* dlogit, int64_t ldd, float* stats, void* stream) {
   if (!logit || !dlogit || !stats || n_agent < 1 || n_demo < 1 || ld < 1 || ldd < 1) { phc_set_error("phc_disc_logit_grad: bad arguments"); return PHC_ERR_INVALID_ARG; }
-  disc_logit_grad_kernel<<<ew_grid(n_agent + n_demo), 256, 0, ST(stream)>>>(logit, ld, n_agent, n_demo, coef, dlogit, ldd, stats); phc_count_launches(1);
+  disc_logit_grad_kernel<<<ew_grid(n_agent + n_demo), 256, 0, ST(stream)>>>(logit, ld, n_agent, n_demo, coef, dlogit, ldd, stats, next_stat_slot()); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "disc_logit_grad_kernel");
 }
 
@@ -703,7 +785,7 @@ extern "C" int phc_relu_mask_row(const float* h, int64_t ldh, const float* w, in
 extern "C" int phc_scale_sumsq(float* x, int64_t ld, int64_t n, int32_t d, float alpha, float* stat, void* stream) {
   if (!x || !stat || n < 0 || d < 1 || ld < d) { phc_set_error("phc_scale_sumsq: bad arguments"); return PHC_ERR_INVALID_ARG; }
   if (n == 0) return PHC_OK;
-  scale_sumsq_kernel<<<ew_grid(n * d), 256, 0, ST(stream)>>>(x, ld, n, d, alpha, stat); phc_count_launches(1);
+  scale_sumsq_kernel<<<ew_grid(n * d), 256, 0, ST(stream)>>>(x, ld, n, d, alpha, stat, next_stat_slot()); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "scale_sumsq_kernel");
 }
 
@@ -711,7 +793,7 @@ extern "C" int phc_axpy2d(const float* x, int64_t ldx, float* y, int64_t ldy, in
                           float* sumsq_stat, void* stream) {
   if (!x || !y || rows < 0 || cols < 1 || ldx < cols || ldy < cols) { phc_set_error("phc_axpy2d: bad arguments"); return PHC_ERR_INVALID_ARG; }
   if (rows == 0) return PHC_OK;
-  axpy2d_kernel<<<ew_grid(rows * cols), 256, 0, ST(stream)>>>(x, ldx, y, ldy, rows, cols, alpha, sumsq_stat); phc_count_launches(1);
+  axpy2d_kernel<<<ew_grid(rows * cols), 256, 0, ST(stream)>>>(x, ldx, y, ldy, rows, cols, alpha, sumsq_stat, sumsq_stat ? next_stat_slot() : 0u); phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "axpy2d_kernel");
 }
 
