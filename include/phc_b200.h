@@ -175,6 +175,12 @@ PHC_API int phc_motion_state(const PhcMotionLib* lib, const int64_t* motion_ids,
                                              task-obs overwrites for far references and the _point_goal update (:783-796) */
 #define PHC_FLAG_CYCLE_MOTION (1u << 10)  /* env.cycle_motion: the launch runs _update_cycle_count (:1076-1079) and the clip
                                              wrap-around of _compute_reset (:1120-1146); pass_time = progress >= max_len - 1 */
+/* env.obs_v: 7 -- the keypoint models (phc_kp_pnn_iccv, phc_kp_mcp_iccv, phc_comp_kp_2): */
+#define PHC_FLAG_TASK_OBS_KP (1u << 13)  /* task obs compute_imitation_observations_v7 (humanoid_im.py:1362-1393, via _compute_task_obs
+                                            :832-853) instead of v6: per sample [diff_pos 3K | diff_vel 3K | ref_pos - root 3K], heading-
+                                            local, no rotations (9 K T columns).  zero_out_far overwrites positions of bodies 1.. and every
+                                            velocity (:834-845); occlusion overwrites the position only -- the reference velocity stays
+                                            (:847-851).  Built for <= PHC_LANE_BODIES bodies (PHC_ERR_UNSUPPORTED on the strided kernel). */
 
 #define PHC_MAX_KEY_BODIES 8
 #define PHC_MAX_BODIES 64      /* J + E; up to PHC_LANE_BODIES the staged one-body-per-lane kernels run, beyond it the strided
@@ -221,7 +227,7 @@ typedef struct PhcStepArgs {
   int32_t amp_joints[PHC_MAX_AMP_JOINTS]; /* [num_amp_joints] joint indices (dof_subset / 3) kept in the AMP obs */
   int32_t num_amp_joints;
   /* ---- outputs ---- */
-  float* obs;            /* [N, obs_stride] first 15J-3(+1) self obs then 24*J*T task obs (obs_buf)     */
+  float* obs;            /* [N, obs_stride] first 15J-3(+1) self obs then 24*J*T task obs (9*J*T with PHC_FLAG_TASK_OBS_KP) */
   int64_t obs_stride;    /* floats between rows                                                          */
   float* rew;            /* [N] rew_buf                                                                  */
   float* reward_raw;     /* [N, 5] (4 when power reward is off)                                          */
@@ -281,6 +287,7 @@ typedef struct PhcStepArgs {
 /* Sizes implied by a configuration (so callers can allocate): */
 PHC_API int phc_self_obs_dim(int32_t num_bodies, uint32_t flags);                    /* 1 + 15J - 3          */
 PHC_API int phc_task_obs_dim(int32_t num_bodies, int32_t time_steps);                /* 24 J T               */
+PHC_API int phc_task_obs_dim_flags(int32_t num_bodies, int32_t time_steps, uint32_t flags); /* 9 J T with PHC_FLAG_TASK_OBS_KP, else 24 J T */
 PHC_API int phc_amp_obs_dim(int32_t num_amp_joints, int32_t num_key_bodies, uint32_t flags); /* 13 + 9 nj + 3 nk */
 /* build_amp_observations_robot (humanoid_amp.py:1062-1104): [root_h?, rot6, vel3, ang_vel3, dof_pos[D], dof_vel[D], key 3 nk] */
 PHC_API int phc_amp_obs_dim_robot(int32_t num_dofs, int32_t num_key_bodies, uint32_t flags); /* 13 + 2 D + 3 nk */

@@ -25,6 +25,7 @@ PHC_FLAG_ZERO_OUT_FAR = 1 << 9
 PHC_FLAG_CYCLE_MOTION = 1 << 10
 PHC_FLAG_NO_SPECIALISE = 1 << 11
 PHC_FLAG_SUBSET_REWARD = 1 << 12
+PHC_FLAG_TASK_OBS_KP = 1 << 13
 PHC_ACT_NONE, PHC_ACT_RELU, PHC_ACT_SILU, PHC_ACT_SILU_BWD, PHC_ACT_RELU_BITS, PHC_ACT_MASK_BITS = 0, 1, 2, 3, 4, 5
 PHC_MAX_KEY_BODIES = 8
 PHC_MAX_BODIES = 64
@@ -108,6 +109,7 @@ SIGNATURES = {
     "phc_motion_state": (C.c_int, [C.POINTER(PhcMotionLib), _p, _p, _p, C.c_int64, C.POINTER(PhcMotionStateOut), _p]),
     "phc_self_obs_dim": (C.c_int, [C.c_int32, C.c_uint32]),
     "phc_task_obs_dim": (C.c_int, [C.c_int32, C.c_int32]),
+    "phc_task_obs_dim_flags": (C.c_int, [C.c_int32, C.c_int32, C.c_uint32]),
     "phc_amp_obs_dim": (C.c_int, [C.c_int32, C.c_int32, C.c_uint32]),
     "phc_env_step": (C.c_int, [C.POINTER(PhcStepArgs), _p]),
     "phc_env_step_fast_launches": (C.c_int64, []),

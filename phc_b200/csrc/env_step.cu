@@ -57,7 +57,8 @@ __host__ __device__ inline StepLayout make_layout(int J, int T, int body_stride,
 // kFastFlags, pose cache on, no env mask, per-env motion records given, every row movable as a TMA bulk copy, no ref_*
 // side buffers.  All of that becomes compile-time, so the flag tests, the non-cache reward path, the row-store fallbacks and
 // their predicates / branches leave the instruction stream (the arithmetic is the same code, operation for operation).
-template <int T_MAX, int JT, bool GETUP = false, bool FAST = false>
+// KP: the keypoint-only task observation v7 (PHC_FLAG_TASK_OBS_KP) instead of v6; a template parameter for the same reason as GETUP.
+template <int T_MAX, int JT, bool GETUP = false, bool FAST = false, bool KP = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtasPerSm)
 env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const int self_dim, const int amp_dim,
                 const bool alias_obs_rt, const bool state_bulk_ok_rt) {
@@ -505,7 +506,7 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
     for (int c = lane; c < ns; c += 32) o_ext[c] = a.shape_params[(size_t)env * ns + c];
     for (int c = lane; c < nl; c += 32) o_ext[ns + c] = a.limb_weights[(size_t)env * nl + c];
   }
-  // task observation v6 for each of the T reference samples (the self observation above did not need the frames)
+  // task observation (v6, or v7 with KP) for each of the T reference samples (the self observation above did not need the frames)
   mbar_wait(bar_o, 0);
   PHC_TL(4);
   float* const g_cache = (FAST || a.ref_cache) ? a.ref_cache + (size_t)env * BS : nullptr;
@@ -538,7 +539,7 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
       }
       if (!tracked) continue;          // env.trackBodies: only the tracked bodies have task-observation columns
       BodyRec ro = ref;                // what the observation sees as reference (the cache / ref_* buffers keep `ref`)
-      if (zof && t == 0) {             // humanoid_im.py:783-796
+      if (zof && t == 0) {             // humanoid_im.py:783-796 (v7: :834-845, the same overwrites of the columns it has)
         const V3 dr = root_p - rroot;
         const float dist = sqrtf(dr.x * dr.x + dr.y * dr.y + dr.z * dr.z);
         if (dist > a.close_distance) {       // far from the reference: it collapses onto the simulated pose (root position excepted)
@@ -551,7 +552,15 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
         if (lane == 0) a.point_goal[env] = dist;
       }
       if (!FAST && a.occlusion && t == 0 && a.occlusion[(size_t)env * K + slot]) {   // _occl_training (humanoid_im.py:797-804)
-        ro.p = sim.p; ro.q = sim.q; ro.v = sim.v; ro.w = sim.w;
+        ro.p = sim.p; ro.q = sim.q;
+        if (!KP) { ro.v = sim.v; ro.w = sim.w; }      // v7 (:847-851) keeps the reference velocity of an occluded body
+      }
+      if (KP) {         // compute_imitation_observations_v7 (humanoid_im.py:1362-1393): [diff_pos | diff_vel | ref_pos - root] per sample
+        float* tb = s_obs + self_dim + t * 9 * K;
+        st3(tb + 3 * slot, qrot_z(hinv, ro.p - sim.p));
+        st3(tb + 3 * K + 3 * slot, qrot_z(hinv, ro.v - sim.v));
+        st3(tb + 6 * K + 3 * slot, qrot_z(hinv, ro.p - root_p));
+        continue;
       }
       float* tb = s_obs + self_dim + t * 24 * K;
       st3(tb + 3 * slot, qrot_z(hinv, ro.p - sim.p));
@@ -616,6 +625,7 @@ extern "C" int phc_self_obs_dim(int32_t J, uint32_t flags) {
   return ((flags & PHC_FLAG_ROOT_HEIGHT_OBS) ? 1 : 0) + 15 * J - 3;
 }
 extern "C" int phc_task_obs_dim(int32_t J, int32_t T) { return 24 * J * T; }
+extern "C" int phc_task_obs_dim_flags(int32_t J, int32_t T, uint32_t flags) { return ((flags & PHC_FLAG_TASK_OBS_KP) ? 9 : 24) * J * T; }
 extern "C" int phc_amp_obs_dim(int32_t nj, int32_t nk, uint32_t flags) {
   return ((flags & PHC_FLAG_ROOT_HEIGHT_OBS) ? 1 : 0) + 12 + 9 * nj + 3 * nk;
 }
@@ -682,10 +692,13 @@ extern "C" int phc_env_step(const PhcStepArgs* a, void* stream) {
     if (seen != a->num_track) { phc_set_error("phc_env_step: track_slot must name exactly num_track bodies"); return PHC_ERR_INVALID_ARG; }
   }
   if (a->occlusion && a->num_track > 0) { phc_set_error("phc_env_step: occlusion training needs every body tracked (the reference indexes random_occlu_idx by body id, humanoid_im.py:1181)"); return PHC_ERR_UNSUPPORTED; }
+  const bool kp = (a->flags & PHC_FLAG_TASK_OBS_KP) != 0;
+  if (kp && wide) { phc_set_error("phc_env_step: the keypoint task observation (PHC_FLAG_TASK_OBS_KP) is built for <= 32-body humanoids"); return PHC_ERR_UNSUPPORTED; }
+  if (kp && getup && J != 24) { phc_set_error("phc_env_step: the keypoint task observation with zero_out_far / cycle_motion is built for 24-body SMPL"); return PHC_ERR_UNSUPPORTED; }
   const bool widened = a->num_track > 0 || a->occlusion || n_shape > 0 || n_limb > 0 || (a->flags & PHC_FLAG_SUBSET_REWARD);
   if (widened && (wide || E > 0)) { phc_set_error("phc_env_step: tracked-body subsets / occlusion / shape columns are built for <= 32-body humanoids without extend bodies"); return PHC_ERR_UNSUPPORTED; }
   const int self_dim = phc_self_obs_dim(J, a->flags) + n_shape + n_limb;
-  const int obs_dim = self_dim + phc_task_obs_dim(a->num_track > 0 ? a->num_track : J, T);
+  const int obs_dim = self_dim + phc_task_obs_dim_flags(a->num_track > 0 ? a->num_track : J, T, a->flags);
   const int amp_dim = !a->amp_out ? 0 : (DR > 0 ? phc_amp_obs_dim_robot(DR, a->num_key_bodies, a->flags)
                                                  : phc_amp_obs_dim(a->num_amp_joints, a->num_key_bodies, a->flags));
   if (a->obs_stride < obs_dim) { phc_set_error("phc_env_step: obs_stride smaller than the observation"); return PHC_ERR_INVALID_ARG; }
@@ -741,7 +754,13 @@ extern "C" int phc_env_step(const PhcStepArgs* a, void* stream) {
     ++g_fast_launches;
     return phc_env_step_fast_launch(a, amp_dim, pdl_allowed ? 1 : 0, stream);
   }
-  if (fast) { PHC_LAUNCH_STEP(1, 24, false, true); ++g_fast_launches; }
+  if (kp) {            // PHC_FLAG_TASK_OBS_KP is not in kFastFlags: keypoint launches never take the FAST paths
+    if (getup) PHC_LAUNCH_STEP(1, 24, true, false, true);
+    else if (T == 1 && J == 24 && E == 0 && DR == 0) PHC_LAUNCH_STEP(1, 24, false, false, true);
+    else if (T == 1) PHC_LAUNCH_STEP(1, 0, false, false, true);
+    else PHC_LAUNCH_STEP(4, 0, false, false, true);
+  }
+  else if (fast) { PHC_LAUNCH_STEP(1, 24, false, true); ++g_fast_launches; }
   else if (getup && J == 24) PHC_LAUNCH_STEP(1, 24, true);                      // env_im_getup_mcp.yaml
   else if (getup) PHC_LAUNCH_STEP(1, 0, true);
   else if (T == 1 && J == 24 && E == 0 && DR == 0) PHC_LAUNCH_STEP(1, 24, false);   // SMPL

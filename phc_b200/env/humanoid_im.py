@@ -136,6 +136,14 @@ class HumanoidIm:
         if self.cycle_motion_xp or self.zero_out_far_train:
             raise NotImplementedError("cycle_motion_xp / zero_out_far_train (random re-placement, humanoid_im.py:966-980, :1131-1140) "
                                       "are not on the fused path; the shipped getup config has both off")
+        # env.obs_v (_compute_task_obs, humanoid_im.py:772-853): 6 for the shipped yamls, 7 for the keypoint models.  The default is 6
+        # (every shipped yaml sets it) although the reference's own is 1 (humanoid.py:296)
+        self.obs_v = int(env.get("obs_v", 6))
+        if self.obs_v not in (6, 7):
+            fn = {1: "compute_imitation_observations", 2: "compute_imitation_observations_v2", 3: "compute_imitation_observations_v3",
+                  4: "compute_imitation_observations_v6 with the obs_v 4 size", 5: "compute_imitation_observations_v6 + one-hot motion types",
+                  8: "compute_imitation_observations_v8", 9: "compute_imitation_observations_v9"}.get(self.obs_v, "no reference observation")
+            raise NotImplementedError(f"env.obs_v {self.obs_v} ({fn}, humanoid_im.py) is not built; obs_v 6 and 7 (keypoints) are")
 
         # ---- simulator backend: explicit object, the synthetic stand-in for synthetic motion data, or the registered factory ----
         sim = cfg.get("sim_backend", None)
@@ -181,6 +189,8 @@ class HumanoidIm:
         to_ids = lambda lst: [names.index(b) if isinstance(b, str) else int(b) for b in lst]
         track = env.get("trackBodies", None)
         self._track_bodies_id = None if track is None or len(track) in (0, J) else to_ids(track)
+        tracked = self._track_bodies_id if self._track_bodies_id is not None else list(range(J))
+        self._track_bodies = [names[b] for b in tracked] if names else tracked       # humanoid_im.py:64-66 keeps the names
         if "reset_bodies" in env:
             reset_bodies = to_ids(env["reset_bodies"])
         elif self._track_bodies_id is not None and "reset_body_ids" not in env:
@@ -215,7 +225,8 @@ class HumanoidIm:
             ext_pos=self.extend_body_pos_in_parent, zero_out_far=self.zero_out_far, close_distance=self.close_distance,
             far_distance=self.far_distance, cycle_motion=self.cycle_motion, max_episode_length=self.max_episode_length,
             specialise=bool(cfg.get("specialised_step", True)), track_bodies=self._track_bodies_id, full_body_reward=self._full_body_reward,
-            term_use_mean=bool(cfg.get("im_eval", False)) and not bool(env.get("strict_eval", False)))   # humanoid_im.py:1180
+            term_use_mean=bool(cfg.get("im_eval", False)) and not bool(env.get("strict_eval", False)),   # humanoid_im.py:1180
+            obs_v=self.obs_v)
         self._key_body_ids, self._reset_bodies_id, self.dof_subset = key_bodies, reset_bodies, dof_subset
 
         # ---- simulator backend and its tensors (Humanoid._setup_tensors) ---------------------------------------
@@ -314,8 +325,8 @@ class HumanoidIm:
     def get_task_obs_size_detail(self):
         """humanoid_im.py:522-537: what the network builders read from the task."""
         env = self.cfg.get("env", self.cfg)
-        return {"target": self._plan.task_dim, "fut_tracks": self._fut_tracks, "num_traj_samples": self._num_traj_samples, "obs_v": env.get("obs_v", 6),
-                "models_path": env.get("models", []), "num_prim": env.get("num_prim", 2),
+        return {"target": self._plan.task_dim, "fut_tracks": self._fut_tracks, "num_traj_samples": self._num_traj_samples, "obs_v": self.obs_v,
+                "track_bodies": self._track_bodies, "models_path": env.get("models", []), "num_prim": env.get("num_prim", 2),
                 "training_prim": env.get("training_prim", 1), "actors_to_load": env.get("actors_to_load", 2),
                 "has_lateral": env.get("has_lateral", True)}
 
@@ -438,7 +449,7 @@ class HumanoidIm:
         return self.self_obs_buf if env_ids is None else self.self_obs_buf[self._reset_mask.bool()]
 
     def _compute_task_obs(self, env_ids=None, save_buffer=True):
-        """HumanoidIm._compute_task_obs (humanoid_im.py:728-871): task observation (v6) of the selected envs; the ref_body_*
+        """HumanoidIm._compute_task_obs (humanoid_im.py:728-871): task observation (v6 or v7) of the selected envs; the ref_body_*
         side buffers are views of the pose cache the launch refreshes (save_buffer is therefore always honoured)."""
         self._compute_observations(env_ids)
         t = self.obs_buf[:, self._plan.self_dim:]

@@ -252,17 +252,19 @@ class AMPAgent:
         netcfg = cfg["network"] = self._network_spec(cfg["network"])
         if netcfg.get("name", "amp") == "amp_mcp":
             # AMPMCPBuilder (amp_network_mcp_builder.py:33-59): has_softmax defaults to TRUE there (appends nn.Softmax) and
-            # ending_act False strips the final activation.  Both shipped MCP configs set has_softmax: False, ending_act: True
-            # (im_mcp.yaml:15-16, im_mcp_big.yaml:15-16) -- the composer built here; anything else must not be built silently.
-            if bool(netcfg.get("has_softmax", True)) or not bool(netcfg.get("ending_act", True)):
-                raise NotImplementedError("amp_mcp composer: only has_softmax: False with ending_act: True (im_mcp.yaml / im_mcp_big.yaml) "
-                                          "is implemented; set them explicitly in the network config")
+            # ending_act False strips the final activation.  The shipped MCP configs set has_softmax: False with ending_act: True
+            # (im_mcp.yaml:15-16, im_mcp_big.yaml:15-16); phc_comp_kp_2 runs im_mcp_big with ending_act: False (a linear head).
+            # The softmax composer must not be built silently.
+            if bool(netcfg.get("has_softmax", True)):
+                raise NotImplementedError("amp_mcp composer: only has_softmax: False (im_mcp.yaml / im_mcp_big.yaml) is implemented; "
+                                          "set it explicitly in the network config")
         self.model = AMPNetwork(self.obs_dim, self.actions_num, self.amp_obs_dim, netcfg["mlp"]["units"],
                                 netcfg["disc"]["units"], netcfg["mlp"]["activation"], netcfg.get("sigma_init", -2.9),
                                 device=self.device, seed=int(cfg["seed"]),
                                 # network.name of the yaml: amp (im.yaml), amp_pnn (im_pnn.yaml), amp_mcp (im_mcp.yaml)
                                 kind=netcfg.get("name", "amp"), num_prim=int(netcfg.get("num_prim", task_detail(task, "num_prim", 4))),
-                                training_prim=int(netcfg.get("training_prim", task_detail(task, "training_prim", 0))))
+                                training_prim=int(netcfg.get("training_prim", task_detail(task, "training_prim", 0))),
+                                ending_act=bool(netcfg.get("ending_act", True)))
         if self.multi_gpu:
             D.broadcast_params(self.model.params, 0)
             self.model._lo_version = -1                 # the collective wrote the bucket behind torch's version counter

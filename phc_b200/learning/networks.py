@@ -72,11 +72,11 @@ class AMPNetwork:
 
     def __init__(self, obs_dim: int, action_dim: int, amp_dim: int, units: Sequence[int] = (1024, 512),
                  disc_units: Sequence[int] = (1024, 512), activation: str = "relu", sigma_init: float = -2.9,
-                 device="cuda:0", seed: int = 0, kind: str = "amp", num_prim: int = 4, training_prim: int = 0):
+                 device="cuda:0", seed: int = 0, kind: str = "amp", num_prim: int = 4, training_prim: int = 0, ending_act: bool = True):
         """kind: 'amp' (AMPBuilder, actor_mlp + mu), 'amp_pnn' (AMPPNNBuilder: `num_prim` independent actor columns
         `pnn.actors.K`, column `training_prim` is the one evaluated / trained -- pnn.py:11-131, amp_network_pnn_builder.py:23-87)
         or 'amp_mcp' (AMPMCPBuilder: `composer` MLP whose `action_dim` = num_prim outputs keep the final ReLU --
-        amp_network_mcp_builder.py:23-91)."""
+        amp_network_mcp_builder.py:23-91; ending_act False strips that ReLU, :58-59)."""
         if activation not in ("relu", "silu"):
             raise NotImplementedError(f"activation {activation!r}: the shipped configs use relu and silu")
         self.activation = activation        # mlp.activation; the discriminator is relu in every shipped config
@@ -91,7 +91,7 @@ class AMPNetwork:
             self.actor = self.pnn_actors[training_prim]
             actor_stacks = self.pnn_actors
         elif kind == "amp_mcp":
-            st = MLPStack("composer", f"composer.{2 * n_h}", obs_dim, units, action_dim, head_relu=True, activation=activation)
+            st = MLPStack("composer", f"composer.{2 * n_h}", obs_dim, units, action_dim, head_relu=ending_act, activation=activation)
             self.actor, actor_stacks = st, [st]
         else:
             self.actor = MLPStack("actor_mlp", "mu", obs_dim, units, action_dim, activation=activation)

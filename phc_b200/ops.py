@@ -247,15 +247,20 @@ class EnvStepConfig:
     # observation (None = all) and whether the tracking reward still averages over every body
     track_bodies: Optional[Sequence[int]] = None
     full_body_reward: bool = True
+    # env.obs_v: 6 = compute_imitation_observations_v6 (24 columns per tracked body and sample), 7 = the keypoint-only v7 of the
+    # keypoint models (9 columns: position / velocity differences and reference positions, humanoid_im.py:1362-1393)
+    obs_v: int = 6
 
     def flags(self) -> int:
+        if self.obs_v not in (6, 7):
+            raise NotImplementedError(f"obs_v {self.obs_v}: only the task observations v6 and v7 (keypoints) are built")
         f = 0
         for on, bit in ((self.upright, PHC_FLAG_UPRIGHT), (self.local_root_obs, PHC_FLAG_LOCAL_ROOT_OBS),
                         (self.root_height_obs, PHC_FLAG_ROOT_HEIGHT_OBS), (self.power_reward, PHC_FLAG_POWER_REWARD),
                         (self.early_term, PHC_FLAG_EARLY_TERM), (self.no_collision, PHC_FLAG_NO_COLLISION),
                         (self.term_use_mean, PHC_FLAG_TERM_USE_MEAN), (self.zero_out_far, _lib.PHC_FLAG_ZERO_OUT_FAR),
                         (self.cycle_motion, _lib.PHC_FLAG_CYCLE_MOTION), (not self.specialise, _lib.PHC_FLAG_NO_SPECIALISE),
-                        (not self.full_body_reward, _lib.PHC_FLAG_SUBSET_REWARD)):
+                        (not self.full_body_reward, _lib.PHC_FLAG_SUBSET_REWARD), (self.obs_v == 7, _lib.PHC_FLAG_TASK_OBS_KP)):
             if on:
                 f |= bit
         return f
@@ -320,7 +325,7 @@ class EnvStepPlan:
         ns = 0 if shape_params is None else int(shape_params.shape[1])
         nl = 0 if limb_weights is None else int(limb_weights.shape[1])
         self.self_dim = lib.phc_self_obs_dim(J, flags) + ns + nl
-        self.task_dim = lib.phc_task_obs_dim(K, cfg.time_steps)
+        self.task_dim = lib.phc_task_obs_dim_flags(K, cfg.time_steps, flags)
         self.obs_dim = self.self_dim + self.task_dim
         robot = mlib.num_dofs > 0
         joints = [] if robot else cfg.amp_joint_list(J)
