@@ -181,6 +181,18 @@ PHC_API int phc_motion_state(const PhcMotionLib* lib, const int64_t* motion_ids,
                                             local, no rotations (9 K T columns).  zero_out_far overwrites positions of bodies 1.. and every
                                             velocity (:834-845); occlusion overwrites the position only -- the reference velocity stays
                                             (:847-851).  Built for <= PHC_LANE_BODIES bodies (PHC_ERR_UNSUPPORTED on the strided kernel). */
+/* env.getup_schedule -- HumanoidImGetup / HumanoidImMCPGetup (phc/env/tasks/humanoid_im_getup.py), recovery episodes: */
+#define PHC_FLAG_RECOVERY (1u << 14)     /* the launch runs _update_recovery_count of pre_physics_step (:198-201): recovery_counter =
+                                            max(counter - 1, 0), written back; then, after the reset test (and the cycle_motion override),
+                                            every env with counter > 0 gets reset = terminate = 0 -- also when the clip ran out (pass_time)
+                                            -- and progress - 1 written back (:203-210).  Reward and reset see the incremented progress, the
+                                            observation the decremented one (humanoid.py:1634-1647), so the ref_cache contract below holds.
+                                            Step launches of time_steps 1, spherical-joint humanoids only (PHC_ERR_UNSUPPORTED otherwise);
+                                            PHC_ERR_INVALID_ARG with PHC_FLAG_OBS_ONLY or a NULL recovery_counter. */
+#define PHC_FLAG_AMP_CURRENT (1u << 15)  /* with PHC_FLAG_OBS_ONLY only: the observation-only launch also writes the AMP vector of the CURRENT
+                                            simulator state (the row a step launch writes for the same state, bit for bit) into slot
+                                            *ring_head (ring_head given) or slot 0 of amp_out: HumanoidAMP._compute_amp_observations(env_ids)
+                                            (humanoid_amp.py:672-707) of the get-up reset path.  Same shapes as PHC_FLAG_RECOVERY. */
 
 #define PHC_MAX_KEY_BODIES 8
 #define PHC_MAX_BODIES 64      /* J + E; up to PHC_LANE_BODIES the staged one-body-per-lane kernels run, beyond it the strided
@@ -282,6 +294,10 @@ typedef struct PhcStepArgs {
   int32_t num_shape;
   const float* limb_weights;
   int32_t num_limb;
+  /* ---- PHC_FLAG_RECOVERY (appended; ignored when the flag is clear) ----
+   * _recovery_counter [N] of HumanoidImGetup (humanoid_im_getup.py:61), read and rewritten by the launch.  With the flag set the
+   * launch also WRITES progress (declared const above for every other launch): progress - 1 for the envs still recovering. */
+  int32_t* recovery_counter;
 } PhcStepArgs;
 
 /* Sizes implied by a configuration (so callers can allocate): */
@@ -301,6 +317,30 @@ PHC_API int64_t phc_env_step_fast_launches(void);
 /* phc_env_step is launched with programmatic stream serialisation (PDL): its CTAs may become resident, and set up their shared
  * memory barriers, while the previous kernel of the stream is finishing; the kernel executes griddepcontrol.wait before its first
  * global-memory access, so ordering is exactly that of a plain launch.  PHC_ENV_PDL=0 in the environment switches the attribute off. */
+
+/* ------------------------------------------------------------------------------------------------------------
+ * Get-up schedule (HumanoidImGetup, phc/env/tasks/humanoid_im_getup.py): reset selection of the envs with mask != 0, in ONE
+ * launch and without a host sync (CUDA-graph capturable), in the order of _reset_actors (:135-182):
+ *   1. available[assignment[e]] = 0 for every masked env (assignments are never cleared: a stale one frees a state another env
+ *      may hold, as in the reference);
+ *   2. recovery envs: u_rec[e] < *p_rec and terminate[e] == 1 -> counter = recovery_steps, simulator state untouched;
+ *   3. fall envs, among the rest: u_fall[e] < *p_fall.  The k-th fall env in ascending env order takes the k-th state s with
+ *      available[s] == 0 in the order of perm (a permutation of [0, P)): body_state[e, 0] = fall_root[s] (13 floats),
+ *      dof_state[e] = (fall_dof_pos[s], 0), counter = recovery_steps, available[s] = 1, assignment[e] = s;
+ *   4. everything else: ref_init[e] = 1 (feed it to phc_reset_bookkeeping / phc_set_env_state / phc_amp_obs_demo) and counter = 0;
+ *   5. progress / reset / terminate = 0 for fall and recovery envs (phc_reset_bookkeeping clears the ref-init ones).
+ * ref_init / fall (int64 0/1) are written for every env (0 outside the mask).  torch.bernoulli(p) == 1 is u < p; perm drawn uniformly
+ * gives the law of available_ids[randperm(n)].  p_rec / p_fall live in device memory so that a captured launch sees schedule
+ * changes.  The bank size P must equal N (then a fall env always finds a free state).  D = dofs per env. */
+PHC_API int phc_getup_reset(const int64_t* mask, const int64_t* terminate_in, const float* u_rec, const float* u_fall, const int64_t* perm,
+                    const float* p_rec, const float* p_fall, int32_t recovery_steps, const float* fall_root /* [P,13] */,
+                    const float* fall_dof_pos /* [P,D] */, int64_t num_states, int64_t* available, int64_t* assignment,
+                    int32_t* recovery_counter, int64_t n, float* body_state, int32_t bodies_per_env, float* dof_state, int32_t num_dofs,
+                    int64_t* progress, int64_t* reset, int64_t* terminate, int64_t* ref_init, int64_t* fall, void* stream);
+/* _init_amp_obs_default (humanoid_amp.py:570-573) on the AMP ring: for every env with mask != 0, every slot of its ring row =
+ * slot *head (the newest vector, e.g. what a PHC_FLAG_AMP_CURRENT launch wrote). */
+PHC_API int phc_amp_ring_fill(float* ring, int64_t ring_stride, int64_t n, int32_t num_steps, int32_t amp_dim, const int32_t* head_dev,
+                      const int64_t* mask, void* stream);
 
 /* build_amp_obs_demo (humanoid_amp.py:253-284) and the history re-initialisation of _init_amp_obs_ref
  * (:575-603): AMP observations of the REFERENCE motion at t0 - (first_step + k)*dt, k = 0..num_steps-1,

@@ -26,6 +26,8 @@ PHC_FLAG_CYCLE_MOTION = 1 << 10
 PHC_FLAG_NO_SPECIALISE = 1 << 11
 PHC_FLAG_SUBSET_REWARD = 1 << 12
 PHC_FLAG_TASK_OBS_KP = 1 << 13
+PHC_FLAG_RECOVERY = 1 << 14
+PHC_FLAG_AMP_CURRENT = 1 << 15
 PHC_ACT_NONE, PHC_ACT_RELU, PHC_ACT_SILU, PHC_ACT_SILU_BWD, PHC_ACT_RELU_BITS, PHC_ACT_MASK_BITS = 0, 1, 2, 3, 4, 5
 PHC_MAX_KEY_BODIES = 8
 PHC_MAX_BODIES = 64
@@ -72,7 +74,7 @@ class PhcStepArgs(C.Structure):
         ("close_distance", C.c_float), ("far_distance", C.c_float), ("max_episode_length", C.c_int32), ("point_goal", _p),
         ("cycle_phase", _p), ("mpjpe", _p), ("body_pos_gt", _p), ("ring_head", _p),
         ("num_track", C.c_int32), ("track_slot", C.c_int8 * PHC_MAX_BODIES), ("occlusion", _p), ("shape_params", _p), ("num_shape", C.c_int32),
-        ("limb_weights", _p), ("num_limb", C.c_int32),
+        ("limb_weights", _p), ("num_limb", C.c_int32), ("recovery_counter", _p),
     ]
 
 
@@ -122,6 +124,9 @@ SIGNATURES = {
     "phc_launch_count_add": (None, [C.c_int64]),
     "phc_amp_window_export": (C.c_int, [_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, C.c_int32, _p, C.c_int64, _p]),
     "phc_set_env_state": (C.c_int, [C.POINTER(PhcMotionLib), _p, _p, _p, _p, C.c_int64, _p, C.c_int32, _p, _p]),
+    "phc_getup_reset": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, C.c_int32, _p, _p, C.c_int64, _p, _p, _p, C.c_int64, _p, C.c_int32, _p,
+                                  C.c_int32, _p, _p, _p, _p, _p, _p]),
+    "phc_amp_ring_fill": (C.c_int, [_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _p, _p, _p]),
     "phc_gae": (C.c_int, [_p, _p, _p, _p, C.c_int32, C.c_int64, C.c_float, C.c_float, _p, _p, _p]),
     "phc_adv_norm_workspace_bytes": (C.c_int64, [C.c_int64]),
     "phc_adv_norm": (C.c_int, [_p, _p, C.c_int64, C.c_int32, _p, _p, _p]),

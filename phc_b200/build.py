@@ -30,6 +30,7 @@ SOURCES = {
     "env_step.cu": ["-fmad=false"] if os.environ.get("PHC_ENV_FMAD", "1") == "0" else [],
     "env_step_fast.cu": [],
     "env_step_wide.cu": [],
+    "getup.cu": [],
     "motion.cu": ["-fmad=false"],
     "motion_wide.cu": ["-fmad=false"],
     "motion_load.cu": ["-fmad=false"],

@@ -58,7 +58,10 @@ __host__ __device__ inline StepLayout make_layout(int J, int T, int body_stride,
 // side buffers.  All of that becomes compile-time, so the flag tests, the non-cache reward path, the row-store fallbacks and
 // their predicates / branches leave the instruction stream (the arithmetic is the same code, operation for operation).
 // KP: the keypoint-only task observation v7 (PHC_FLAG_TASK_OBS_KP) instead of v6; a template parameter for the same reason as GETUP.
-template <int T_MAX, int JT, bool GETUP = false, bool FAST = false, bool KP = false>
+// REC: the get-up schedule (HumanoidImGetup, humanoid_im_getup.py): PHC_FLAG_RECOVERY on a step launch (recovery counter, reset
+// override, frozen progress) and PHC_FLAG_AMP_CURRENT on the observation-only launch (the AMP vector of the current state); again a
+// template parameter so that every other instantiation keeps its instruction stream.
+template <int T_MAX, int JT, bool GETUP = false, bool FAST = false, bool KP = false, bool REC = false>
 __global__ void __launch_bounds__(kWarpsPerCta * 32, kMinCtasPerSm)
 env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const int self_dim, const int amp_dim,
                 const bool alias_obs_rt, const bool state_bulk_ok_rt) {
@@ -142,6 +145,11 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
 
   // ---- every load that depends only on the env index is issued first (one DRAM round trip for all of them) ----------
   const int64_t progress = a.progress[env];
+  // PHC_FLAG_RECOVERY: _update_recovery_count (humanoid_im_getup.py:198-201) -- the counter after this step's decrement.  An env still
+  // recovering keeps progress - 1 (:209), which is also the progress its observation is built for (humanoid.py:1641-1647)
+  int rcnt = 0;
+  if (REC && (flags & PHC_FLAG_RECOVERY)) { const int c = a.recovery_counter[env]; rcnt = c - 1 < 0 ? 0 : c - 1; }
+  const int64_t progress_o = (REC && rcnt > 0) ? progress - 1 : progress;
   const float t_start = a.start_times[env], t_off = a.start_offsets[env];
   const V3 goff = v3(a.global_offset[3 * env + 0], a.global_offset[3 * env + 1], a.global_offset[3 * env + 2]);
   float m_len, m_dt;
@@ -235,7 +243,7 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
     for (int t = 0; t < T_MAX; ++t) {
       if (t < T) {
         // ((progress + 1) * dt [+ t * traj_dt] + start + offset), humanoid_im.py:744-752
-        float tn = PHC_MUL((float)(progress + 1), a.dt);
+        float tn = PHC_MUL((float)(progress_o + 1), a.dt);
         if (T > 1) tn = PHC_ADD(tn, PHC_MUL((float)t, a.traj_dt));
         tn = PHC_ADD(PHC_ADD(tn, t_start_o), t_off_o);
         const Bracket32 b = frame_bracket32(tn, m_len, (int)m_nf, m_dt);
@@ -438,13 +446,16 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
       int64_t reset = pass_time ? 1 : terminated;
       if (GETUP) { if (!pass_time && cc > 0) { reset = 0; terminated = 0; } }
       else if (a.cycle_counter && !pass_time && a.cycle_counter[env] > 0) { reset = 0; terminated = 0; }
+      if (REC && rcnt > 0) { reset = 0; terminated = 0; }      // humanoid_im_getup.py:203-210: not cancelled by pass_time
       a.reset[env] = reset;
       a.terminate[env] = terminated;
     }
   }
 
-  // AMP observation of the simulated character (build_amp_observations_smpl) -> its own staging row
-  if ((FAST || a.amp_out) && !obs_only) {
+  // AMP observation of the simulated character (build_amp_observations_smpl) -> its own staging row; the observation-only launch
+  // writes it only with PHC_FLAG_AMP_CURRENT (the get-up reset path)
+  const bool amp_cur = REC && obs_only && (flags & PHC_FLAG_AMP_CURRENT);
+  if ((FAST || a.amp_out) && (!obs_only || amp_cur)) {
     const int nj = a.num_amp_joints, nk = a.num_key_bodies;
     float* o = s_amp + base0;
     if (lane == 0) {
@@ -474,11 +485,15 @@ env_step_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const 
   // rows leave shared memory as TMA bulk stores (one instruction per row) when source, destination and size are 16-byte
   // granular; otherwise with per-lane coalesced stores; all rows of the env go out together at the end.
   // ring mode with the head on the device (PhcStepArgs.ring_head): this step's vector goes to slot *ring_head of the env's ring
-  float* const g_amp = ((FAST || a.amp_out) && !obs_only)
+  float* const g_amp = ((FAST || a.amp_out) && (!obs_only || amp_cur))
                            ? a.amp_out + (size_t)env * a.amp_out_stride + (a.ring_head ? (size_t)(*a.ring_head) * (size_t)amp_dim : (size_t)0) : nullptr;
   const bool amp_bulk = FAST ? true : (g_amp && !a.amp_hist_in && (amp_dim & 3) == 0 && (reinterpret_cast<uintptr_t>(g_amp) & 15) == 0);
   __syncwarp();   // the reward slots and the simulator block are consumed: the obs row may overwrite them
   PHC_TL(3);
+  if (REC && (flags & PHC_FLAG_RECOVERY) && lane == 0) {     // every lane has read both values: write them back
+    a.recovery_counter[env] = rcnt;
+    if (rcnt > 0) const_cast<int64_t*>(a.progress)[env] = progress_o;
+  }
 
   // ================= phase B: observation row (reads only registers + the observation slots) =================
   if (lane == 0 && has_h) s_obs[0] = root_p.z;
@@ -695,6 +710,17 @@ extern "C" int phc_env_step(const PhcStepArgs* a, void* stream) {
   const bool kp = (a->flags & PHC_FLAG_TASK_OBS_KP) != 0;
   if (kp && wide) { phc_set_error("phc_env_step: the keypoint task observation (PHC_FLAG_TASK_OBS_KP) is built for <= 32-body humanoids"); return PHC_ERR_UNSUPPORTED; }
   if (kp && getup && J != 24) { phc_set_error("phc_env_step: the keypoint task observation with zero_out_far / cycle_motion is built for 24-body SMPL"); return PHC_ERR_UNSUPPORTED; }
+  // get-up schedule (PHC_FLAG_RECOVERY on a step launch, PHC_FLAG_AMP_CURRENT on the observation-only one): the GETUP instantiations
+  const bool recovery = (a->flags & PHC_FLAG_RECOVERY) != 0, amp_cur = (a->flags & PHC_FLAG_AMP_CURRENT) != 0;
+  const bool obs_only_l = (a->flags & PHC_FLAG_OBS_ONLY) != 0;
+  if (recovery && obs_only_l) { phc_set_error("phc_env_step: PHC_FLAG_RECOVERY is for step launches, not the observation-only launch"); return PHC_ERR_INVALID_ARG; }
+  if (recovery && !a->recovery_counter) { phc_set_error("phc_env_step: PHC_FLAG_RECOVERY needs recovery_counter"); return PHC_ERR_INVALID_ARG; }
+  if (amp_cur && (!obs_only_l || !a->amp_out)) { phc_set_error("phc_env_step: PHC_FLAG_AMP_CURRENT needs PHC_FLAG_OBS_ONLY and amp_out"); return PHC_ERR_INVALID_ARG; }
+  if ((recovery || amp_cur) && (T != 1 || E != 0 || DR != 0)) {
+    phc_set_error("phc_env_step: the get-up schedule (PHC_FLAG_RECOVERY / PHC_FLAG_AMP_CURRENT) is built for time_steps 1 and spherical-joint humanoids without extend bodies");
+    return PHC_ERR_UNSUPPORTED;
+  }
+  if ((recovery || amp_cur) && kp && J != 24) { phc_set_error("phc_env_step: the keypoint task observation with the get-up schedule is built for 24-body SMPL"); return PHC_ERR_UNSUPPORTED; }
   const bool widened = a->num_track > 0 || a->occlusion || n_shape > 0 || n_limb > 0 || (a->flags & PHC_FLAG_SUBSET_REWARD);
   if (widened && (wide || E > 0)) { phc_set_error("phc_env_step: tracked-body subsets / occlusion / shape columns are built for <= 32-body humanoids without extend bodies"); return PHC_ERR_UNSUPPORTED; }
   const int self_dim = phc_self_obs_dim(J, a->flags) + n_shape + n_limb;
@@ -754,7 +780,12 @@ extern "C" int phc_env_step(const PhcStepArgs* a, void* stream) {
     ++g_fast_launches;
     return phc_env_step_fast_launch(a, amp_dim, pdl_allowed ? 1 : 0, stream);
   }
-  if (kp) {            // PHC_FLAG_TASK_OBS_KP is not in kFastFlags: keypoint launches never take the FAST paths
+  if (recovery || amp_cur) {      // the flags are not in kFastFlags: get-up launches never take the FAST paths
+    if (kp) PHC_LAUNCH_STEP(1, 24, true, false, true, true);
+    else if (J == 24) PHC_LAUNCH_STEP(1, 24, true, false, false, true);
+    else PHC_LAUNCH_STEP(1, 0, true, false, false, true);
+  }
+  else if (kp) {            // PHC_FLAG_TASK_OBS_KP is not in kFastFlags: keypoint launches never take the FAST paths
     if (getup) PHC_LAUNCH_STEP(1, 24, true, false, true);
     else if (T == 1 && J == 24 && E == 0 && DR == 0) PHC_LAUNCH_STEP(1, 24, false, false, true);
     else if (T == 1) PHC_LAUNCH_STEP(1, 0, false, false, true);

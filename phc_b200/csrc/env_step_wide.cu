@@ -51,6 +51,9 @@ __device__ __forceinline__ Body blend(const float* s0, const float* s1, float bl
 __device__ __forceinline__ void put3(float* d, V3 v) { d[0] = v.x; d[1] = v.y; d[2] = v.z; }
 __device__ __forceinline__ void put6(float* d, TanNorm t) { put3(d, t.t); put3(d + 3, t.n); }
 
+// REC: the get-up schedule (PHC_FLAG_RECOVERY / PHC_FLAG_AMP_CURRENT, semantics at env_step.cu's REC variant); a template parameter so
+// that the plain instantiation keeps its instruction stream.
+template <bool REC = false>
 __global__ void __launch_bounds__(kWarps * 32)
 env_step_wide_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, const int self_dim, const int amp_dim) {
   const int warp = threadIdx.x >> 5, lane = threadIdx.x & 31;
@@ -69,6 +72,10 @@ env_step_wide_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, c
   const float* g_state = a.body_state + (size_t)env * a.bodies_per_env * kRec;
   const float* g_dof = a.dof_state + (size_t)env * D * 2;                  // (pos, vel) interleaved
   const int64_t progress = a.progress[env];
+  // PHC_FLAG_RECOVERY (humanoid_im_getup.py:198-210): counter after the decrement; a recovering env keeps progress - 1 (observation too)
+  int rcnt = 0;
+  if (REC && (flags & PHC_FLAG_RECOVERY)) { const int c = a.recovery_counter[env]; rcnt = c - 1 < 0 ? 0 : c - 1; }
+  const int64_t progress_o = (REC && rcnt > 0) ? progress - 1 : progress;
   const float t_start = a.start_times[env], t_off = a.start_offsets[env];
   const V3 goff = v3(a.global_offset[3 * env + 0], a.global_offset[3 * env + 1], a.global_offset[3 * env + 2]);
   float m_len, m_dt;
@@ -130,7 +137,10 @@ env_step_wide_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, c
   const int base0 = has_h ? 1 : 0;
 
   // ================= reward / reset at the CURRENT motion time (humanoid_im.py:879, :1118) ===========================
-  if (!obs_only) {
+  // (the observation-only launch skips it, and writes the AMP vector below only with PHC_FLAG_AMP_CURRENT: the get-up reset path)
+  const bool amp_cur = REC && obs_only && (flags & PHC_FLAG_AMP_CURRENT);
+  if (!obs_only || amp_cur) {
+   if (!obs_only) {
     const float t_now = PHC_ADD(PHC_ADD(PHC_MUL((float)progress, a.dt), t_start), t_off);
     Bracket32 br;
     br.i0 = 0; br.i1 = 0; br.blend = 0.f;
@@ -231,9 +241,18 @@ env_step_wide_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, c
       }
       int64_t reset = pass_time ? 1 : terminated;
       if (a.cycle_counter && !pass_time && cc > 0) { reset = 0; terminated = 0; }      // cc: this lane's own read (+ update)
+      if (REC && rcnt > 0) { reset = 0; terminated = 0; }      // humanoid_im_getup.py:203-210: not cancelled by pass_time
       a.reset[env] = reset;
       a.terminate[env] = terminated;
     }
+    if (REC && (flags & PHC_FLAG_RECOVERY)) {
+      __syncwarp();          // every lane has read the counter and progress before lane 0 rewrites them
+      if (lane == 0) {
+        a.recovery_counter[env] = rcnt;
+        if (rcnt > 0) const_cast<int64_t*>(a.progress)[env] = progress_o;
+      }
+    }
+   }
 
     // ================= AMP observation of the simulated character -> slot 0 of its window ============================
     if (a.amp_out) {
@@ -286,7 +305,7 @@ env_step_wide_kernel(const __grid_constant__ PhcStepArgs a, const int obs_dim, c
     put3(o_ang + 3 * jj, qrot_z(hinv, sim.w));
   }
   for (int t = 0; t < T; ++t) {                // compute_imitation_observations_v6 (humanoid_im.py:1308-1358)
-    float tn = PHC_MUL((float)(progress + 1), a.dt);
+    float tn = PHC_MUL((float)(progress_o + 1), a.dt);
     if (T > 1) tn = PHC_ADD(tn, PHC_MUL((float)t, a.traj_dt));
     tn = PHC_ADD(PHC_ADD(tn, t_start_o), t_off_o);
     const Bracket32 b = frame_bracket32(tn, m_len, (int)m_nf, m_dt);
@@ -347,7 +366,10 @@ extern "C" void phc_count_launches(int n);
 extern "C" int phc_env_step_wide_launch(const PhcStepArgs* a, int obs_dim, int self_dim, int amp_dim, void* stream) {
   using namespace phc::wide;
   const int grid = (a->num_envs + kWarps - 1) / kWarps;
-  env_step_wide_kernel<<<grid, kWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(*a, obs_dim, self_dim, amp_dim);
+  if (a->flags & (PHC_FLAG_RECOVERY | PHC_FLAG_AMP_CURRENT))
+    env_step_wide_kernel<true><<<grid, kWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(*a, obs_dim, self_dim, amp_dim);
+  else
+    env_step_wide_kernel<<<grid, kWarps * 32, 0, static_cast<cudaStream_t>(stream)>>>(*a, obs_dim, self_dim, amp_dim);
   phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "env_step_wide_kernel launch");
 }

@@ -13,6 +13,8 @@ d.install_on_import()`) that runs before the script's imports:
 `install_on_import()` registers a meta-path hook that waits for the reference modules to be imported and then rebinds
   phc.env.tasks.humanoid_im.HumanoidIm / env.tasks.humanoid_im.HumanoidIm   -> phc_b200.env.humanoid_im.HumanoidIm
   phc.env.tasks.humanoid_im_mcp.HumanoidImMCP (+ short name)                 -> phc_b200.env.humanoid_im_mcp.HumanoidImMCP
+  phc.env.tasks.humanoid_im_getup.HumanoidImGetup (+ short name)            -> phc_b200.env.humanoid_im_getup.HumanoidImGetup
+  phc.env.tasks.humanoid_im_mcp_getup.HumanoidImMCPGetup (+ short name)      -> phc_b200.env.humanoid_im_getup.HumanoidImMCPGetup
   learning.amp_agent.AMPAgent / phc.learning.amp_agent.AMPAgent              -> phc_b200.learning.amp_agent.AMPAgent
   learning.im_amp.IMAmpAgent / phc.learning.im_amp.IMAmpAgent                -> phc_b200.learning.im_amp.IMAmpAgent
 so `IMAmpAgent(AMPAgent)` (learning/im_amp.py) and `eval("HumanoidIm")` resolve to the phc_b200 implementations.  `install()` does
@@ -30,6 +32,10 @@ from typing import Dict, Tuple
 _TARGETS: Dict[Tuple[str, ...], Dict[str, str]] = {
     ("phc.env.tasks.humanoid_im", "env.tasks.humanoid_im"): {"HumanoidIm": "phc_b200.env.humanoid_im:HumanoidIm"},
     ("phc.env.tasks.humanoid_im_mcp", "env.tasks.humanoid_im_mcp"): {"HumanoidImMCP": "phc_b200.env.humanoid_im_mcp:HumanoidImMCP"},
+    # the get-up schedule (env_im_getup_mcp.yaml, env_im_x_getup_mcp.yaml, env_im_x_pnn.yaml)
+    ("phc.env.tasks.humanoid_im_getup", "env.tasks.humanoid_im_getup"): {"HumanoidImGetup": "phc_b200.env.humanoid_im_getup:HumanoidImGetup"},
+    ("phc.env.tasks.humanoid_im_mcp_getup", "env.tasks.humanoid_im_mcp_getup"): {
+        "HumanoidImMCPGetup": "phc_b200.env.humanoid_im_getup:HumanoidImMCPGetup"},
     ("phc.learning.amp_agent", "learning.amp_agent"): {"AMPAgent": "phc_b200.learning.amp_agent:AMPAgent"},
     # run_hydra.py:259 registers `im_amp.IMAmpAgent` as the 'im_amp' algorithm: the mirror keeps eval / _post_step_eval / get_action
     ("phc.learning.im_amp", "learning.im_amp"): {"IMAmpAgent": "phc_b200.learning.im_amp:IMAmpAgent"},

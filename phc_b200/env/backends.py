@@ -13,6 +13,8 @@ physics.  What a backend is (duck typed; `SyntheticSim` in humanoid_im.py and `I
   optional, needed when HumanoidIm has to LOAD motions itself (cfg without `motion_data`):
     skeleton_trees, humanoid_shapes, humanoid_limb_and_weights       what Humanoid keeps per env for MotionLib.load_motions
   optional:
+    generate_fall_states()                 -> (root_states [N, 13], dof_pos [N, D]): the bank of fallen states HumanoidImGetup starts
+                                           episodes from (humanoid_im_getup.py:82-125); required by HumanoidImGetup / HumanoidImMCPGetup
     pd_action_offset / pd_action_scale     Humanoid._build_pd_action_offset_scale (humanoid.py:1331-1380)
     graph_safe = True                      simulate() only enqueues work on the current CUDA stream (CUDA-graph capturable)
 
@@ -80,3 +82,30 @@ class IsaacGymBackend:
         actor_ids = t._humanoid_actor_ids[ids]
         t.gym.set_actor_root_state_tensor_indexed(t.sim, gymtorch.unwrap_tensor(t._root_states), gymtorch.unwrap_tensor(actor_ids), len(actor_ids))
         t.gym.set_dof_state_tensor_indexed(t.sim, gymtorch.unwrap_tensor(t._dof_state), gymtorch.unwrap_tensor(actor_ids), len(actor_ids))
+
+    def generate_fall_states(self):
+        """HumanoidImGetup._generate_fall_states (humanoid_im_getup.py:82-125) on the wrapped task: random unit root rotations at the
+        initial root states, zero dof state, one uniform [-0.5, 0.5) action, 150 physics steps; returns the settled root states (velocities
+        zeroed) and dof positions."""
+        import numpy as np
+        from isaacgym import gymtorch
+        t = self._t
+        N = t.num_envs
+        env_ids = torch.arange(N, device=t.device, dtype=torch.long)
+        root_states = t._initial_humanoid_root_states[env_ids].clone()
+        root_states[..., 3:7] = torch.randn_like(root_states[..., 3:7])
+        root_states[..., 3:7] = torch.nn.functional.normalize(root_states[..., 3:7], dim=-1)
+        t._humanoid_root_states[env_ids] = root_states
+        actor_ids = t._humanoid_actor_ids[env_ids]
+        t.gym.set_actor_root_state_tensor_indexed(t.sim, gymtorch.unwrap_tensor(t._root_states), gymtorch.unwrap_tensor(actor_ids), len(actor_ids))
+        t.gym.set_dof_state_tensor_indexed(t.sim, gymtorch.unwrap_tensor(torch.zeros_like(t._dof_state)), gymtorch.unwrap_tensor(actor_ids),
+                                           len(actor_ids))
+        rand_actions = torch.as_tensor(np.random.uniform(-0.5, 0.5, size=[N, t.get_dof_action_size()]), dtype=torch.float32, device=t.device)
+        t.pre_physics_step(rand_actions)
+        for _ in range(150):
+            t.render()
+            t.gym.simulate(t.sim)
+        t._refresh_sim_tensors()
+        root = t._humanoid_root_states.clone()
+        root[:, 7:13] = 0
+        return root, t._dof_pos.clone()

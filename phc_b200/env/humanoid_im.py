@@ -81,6 +81,18 @@ class SyntheticSim:
         dynamics to reset -- its next snapshot replaces every row anyway -- so there is nothing to do."""
         return
 
+    def generate_fall_states(self, seed: int = 0):
+        """Backend hook of HumanoidImGetup (humanoid_im_getup.py:82-125): a bank of one "fallen" state per env, (root_states [N, 13],
+        dof_pos [N, D]).  The stand-in has no physics to let the characters fall, so the bank is the first snapshot with a seeded random
+        unit root rotation (the reference's randn + normalize, :90-91) and zero root velocities; deterministic for a given seed."""
+        g = torch.Generator().manual_seed(int(seed))
+        root = self.init_state.body_state[:, 0, :].detach().cpu().clone().float()
+        q = torch.randn(root.shape[0], 4, generator=g)
+        root[:, 3:7] = torch.nn.functional.normalize(q, dim=-1)
+        root[:, 7:13] = 0
+        dof_pos = self.init_state.dof_state[..., 0].detach().cpu().clone().float()
+        return root.to(self.device), dof_pos.to(self.device)
+
     def simulate(self, actions: Optional[torch.Tensor]) -> None:
         k = self._k = (self._k + 1) % self._body.shape[0]
         self.rigid_body_state.copy_(self._body[k], non_blocking=True)

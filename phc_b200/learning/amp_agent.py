@@ -505,9 +505,10 @@ class AMPAgent:
         config or PHC_GRAPH_ROLLOUT=0 keeps the eager loop; the phase timer needs the eager loop too)."""
         if not self._graph_rollout or self.timer.enabled:
             return self._play_steps_eager()
-        version = getattr(self.vec_env.env.task, "_motion_version", 0)
+        # the captured launches point at the motion tables and carry _combine_rewards' weights as constants: re-capture when either changes
+        version = (getattr(self.vec_env.env.task, "_motion_version", 0), self._task_reward_w, self._disc_reward_w)
         if self._rollout_graph is not None and version != self._rollout_graph_version:
-            self._rollout_graph = self._rollout_out = None      # the motion tables were re-loaded: the captured launches point at the old ones
+            self._rollout_graph = self._rollout_out = None
             self._rollout_calls = 1
         if self._rollout_graph is not None:
             self._rollout_graph.replay()
@@ -938,6 +939,13 @@ class AMPAgent:
         if (getattr(task, "humanoid_type", "") in ("smpl", "smplh", "smplx") and hasattr(getattr(task, "_motion_data", None), "load_motions")
                 and hasattr(task.sim, "skeleton_trees") and epoch_num > 1 and epoch_num % int(task.shape_resampling_interval) == 1):
             task.resample_motions()
+        # the get-up schedule (amp_agent.py:518-525): fall starts only and the discriminator reward alone until getup_udpate_epoch
+        if getattr(task, "humanoid_type", "") in ("smpl", "smplh", "smplx") and getattr(task, "getup_schedule", False):
+            task.update_getup_schedule(epoch_num, getup_udpate_epoch=task.getup_udpate_epoch)
+            if epoch_num > task.getup_udpate_epoch:
+                self._task_reward_w, self._disc_reward_w = 0.5, 0.5
+            else:
+                self._task_reward_w, self._disc_reward_w = 0, 1
         if self.normalize_input:
             self.running_mean_std_temp = self.running_mean_std.frozen_copy()   # amp_agent.py:527-528
 

@@ -69,6 +69,10 @@ class IMAmpAgent(AMPAgent):
         self.terminate_memory: List[torch.Tensor] = []
         self.mpjpe_all: List[torch.Tensor] = []
         self.curr_stpes, self.success_rate = 0, 0.0
+        # the get-up schedule is off for the sweep (im_amp.py:167-172, :228-232)
+        getup_probs = (task._recovery_episode_prob, task._fall_init_prob) if hasattr(task, "set_getup_probs") else None
+        if getup_probs is not None:
+            task.set_getup_probs(0, 0)
         task.set_eval_mode(True)
         task.begin_seq_motion_samples()
         try:
@@ -81,6 +85,8 @@ class IMAmpAgent(AMPAgent):
                 done_mask, info = self._post_step_eval(step_info, done.clone())
         finally:
             task.set_eval_mode(False)
+            if getup_probs is not None:
+                task.set_getup_probs(*getup_probs)
             if hasattr(lib, "load_motions"):
                 task.resample_motions()                     # back to sampled training clips, every env reset (im_amp.py:226-238)
         self.update_training_data(info["failed_keys"])

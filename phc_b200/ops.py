@@ -290,12 +290,14 @@ class EnvStepPlan:
                  ref_cache: Optional[torch.Tensor] = None, reward_from_cache: bool = False,
                  point_goal: Optional[torch.Tensor] = None, cycle_phase: Optional[torch.Tensor] = None,
                  with_eval_extras: bool = False, ring_head_dev: Optional[torch.Tensor] = None, occlusion: Optional[torch.Tensor] = None,
-                 shape_params: Optional[torch.Tensor] = None, limb_weights: Optional[torch.Tensor] = None):
+                 shape_params: Optional[torch.Tensor] = None, limb_weights: Optional[torch.Tensor] = None, amp_current: bool = False):
         """ref_cache: [N, body_stride] pose cache (PhcStepArgs.ref_cache): every run() stores the reference pose interpolated
         for the first observation sample; reward_from_cache=True makes run() take the reward-time reference pose from it
         (valid for HumanoidIm's step / reset sequence, see include/phc_b200.h).
         amp_ring=True: `amp_obs_buf` is a ring -- each run() writes only the newest vector into slot `ring_head`
         (advance with advance_ring() before the step); otherwise the reference's window shift is done in the kernel.
+        amp_current=True (with obs_only): the launch also writes the AMP vector of the current simulator state into the newest slot
+        (PHC_FLAG_AMP_CURRENT, the get-up reset path); the window is not shifted.
         ring_head_dev: int32 [1] device tensor holding the ring head (PhcStepArgs.ring_head): the slot is then read on the device and
         advance_ring() is a one-thread kernel, so consecutive steps differ in nothing the host passes (CUDA-graph capturable)."""
         lib = _lib.load()
@@ -316,6 +318,10 @@ class EnvStepPlan:
             assert dof_force.shape == (N, D)
         self.N, self.J = N, J
         flags = cfg.flags() | (_lib.PHC_FLAG_OBS_ONLY if obs_only else 0)
+        if amp_current:
+            assert obs_only and with_amp, "amp_current is an option of the observation-only launch with an AMP buffer"
+            flags |= _lib.PHC_FLAG_AMP_CURRENT
+            amp_shift = False
         if reward_from_cache:
             assert ref_cache is not None and not obs_only
             flags |= _lib.PHC_FLAG_REWARD_FROM_CACHE
@@ -470,6 +476,14 @@ class EnvStepPlan:
         self._args_ref = C.byref(a)
         self.refresh_motion_params()
 
+    def set_recovery_counter(self, counter: torch.Tensor) -> None:
+        """Turn on the get-up schedule's recovery episodes (PHC_FLAG_RECOVERY): every later run() decrements `counter` (int32 [N],
+        HumanoidImGetup._recovery_counter) and keeps envs with a running counter from resetting or advancing their progress."""
+        self._keep["recovery_counter"] = _req(counter, torch.int32, "recovery_counter", self.device)
+        assert counter.shape == (self.N,)
+        self.args.recovery_counter = counter.data_ptr()
+        self.args.flags |= _lib.PHC_FLAG_RECOVERY
+
     def set_motion_lib(self, mlib: PackedMotionLib) -> None:
         """Re-point the plan at a re-loaded motion library of the same character (HumanoidIm.resample_motions): new frame tables,
         new per-env motion records; every other pointer of the launch stays."""
@@ -528,6 +542,47 @@ def amp_obs_demo(mlib: PackedMotionLib, cfg: EnvStepConfig, motion_ids: torch.Te
                                              None if only_where is None else _req(only_where, torch.int64, "only_where", dev).data_ptr(),
                                              int(slot_offset), _ptr(slot_offset_dev), _stream()), "phc_amp_obs_demo")
     return out
+
+
+def getup_reset(mask: torch.Tensor, terminate_in: torch.Tensor, u_rec: torch.Tensor, u_fall: torch.Tensor, perm: torch.Tensor,
+                p_rec: torch.Tensor, p_fall: torch.Tensor, recovery_steps: int, fall_root: torch.Tensor, fall_dof_pos: torch.Tensor,
+                available: torch.Tensor, assignment: torch.Tensor, recovery_counter: torch.Tensor, body_state: torch.Tensor,
+                dof_state: torch.Tensor, progress: torch.Tensor, reset: torch.Tensor, terminate: torch.Tensor, ref_init: torch.Tensor,
+                fall: torch.Tensor) -> None:
+    """phc_getup_reset: the reset selection of HumanoidImGetup._reset_actors (humanoid_im_getup.py:135-182) for the envs with mask != 0.
+    Writes ref_init / fall (int64 0/1 masks), the fall envs' root record and dof state, the bank marks, assignments and counters."""
+    lib = _lib.load()
+    dev = body_state.device
+    i64, f32 = torch.int64, torch.float32
+    n = int(mask.shape[0])
+    D = int(dof_state.shape[1])
+    for t, dt, name in ((mask, i64, "mask"), (terminate_in, i64, "terminate_in"), (u_rec, f32, "u_rec"), (u_fall, f32, "u_fall"),
+                        (perm, i64, "perm"), (p_rec, f32, "p_rec"), (p_fall, f32, "p_fall"), (fall_root, f32, "fall_root"),
+                        (fall_dof_pos, f32, "fall_dof_pos"), (available, i64, "available"), (assignment, i64, "assignment"),
+                        (recovery_counter, torch.int32, "recovery_counter"), (body_state, f32, "body_state"), (dof_state, f32, "dof_state"),
+                        (progress, i64, "progress"), (reset, i64, "reset"), (terminate, i64, "terminate"), (ref_init, i64, "ref_init"),
+                        (fall, i64, "fall")):
+        _req(t, dt, name, dev)
+    P = int(fall_root.shape[0])
+    assert fall_root.shape == (P, 13) and fall_dof_pos.shape == (P, D) and perm.shape == (P,) and available.shape == (P,)
+    assert body_state.shape[0] == n and dof_state.shape == (n, D, 2)
+    for t in (terminate_in, u_rec, u_fall, assignment, recovery_counter, progress, reset, terminate, ref_init, fall):
+        assert t.shape == (n,)
+    _lib.check(lib.phc_getup_reset(mask.data_ptr(), terminate_in.data_ptr(), u_rec.data_ptr(), u_fall.data_ptr(), perm.data_ptr(),
+                                   p_rec.data_ptr(), p_fall.data_ptr(), int(recovery_steps), fall_root.data_ptr(), fall_dof_pos.data_ptr(), P,
+                                   available.data_ptr(), assignment.data_ptr(), recovery_counter.data_ptr(), n, body_state.data_ptr(),
+                                   int(body_state.shape[1]), dof_state.data_ptr(), D, progress.data_ptr(), reset.data_ptr(),
+                                   terminate.data_ptr(), ref_init.data_ptr(), fall.data_ptr(), _stream()), "phc_getup_reset")
+
+
+def amp_ring_fill(ring: torch.Tensor, head, mask: torch.Tensor) -> None:
+    """phc_amp_ring_fill: every slot of the masked envs' AMP rows = the newest slot (`head`: the int32 [1] device ring head, or None
+    for a newest-first window whose newest slot is 0) -- _init_amp_obs_default (humanoid_amp.py:570-573)."""
+    lib = _lib.load()
+    n, S, A = ring.shape
+    _req(ring, torch.float32, "ring")
+    _req(mask, torch.int64, "mask", ring.device)
+    _lib.check(lib.phc_amp_ring_fill(ring.data_ptr(), ring.stride(0), n, S, A, _ptr(head), mask.data_ptr(), _stream()), "phc_amp_ring_fill")
 
 
 def amp_window_export(ring: torch.Tensor, head, out: torch.Tensor) -> torch.Tensor:
