@@ -7,13 +7,15 @@
 // per k-step D += A_lo*B_hi, D += A_hi*B_lo, D += A_hi*B_hi.  The dropped A_lo*B_lo term is <= 2^-20 |ab|.
 //
 // wgmma reads tf32 operands from shared memory in K-major order only, so the CTA's threads stage every k-block themselves:
-// global -> registers (16-byte loads for k-contiguous operands, a transposing gather for mn-contiguous ones) -> hi / lo split ->
-// shared memory in the canonical no-swizzle K-major layout (8-row x 16-byte core matrices; LBO = 128 B between the core
-// matrices along K, SBO = BK * 32 B between 8-row groups).  Two shared-memory buffers: the loads and the split of k-block i + 1
-// run while the asynchronous wgmmas of k-block i execute.
+// global -> registers (16-byte loads for both operand orders) -> hi / lo split -> shared memory in the canonical no-swizzle
+// K-major layout (8-row x 16-byte core matrices; LBO = 128 B between the core matrices along K, SBO = BK * 32 B between 8-row
+// groups).  The k-loop is a software pipeline over a ring of three shared-memory stages: while the wgmmas of k-block i run,
+// k-block i + 1 is split and stored into the next stage, and then the global loads of k-block i + 2 are issued and stay in
+// flight across the k-block boundary.  wgmma.wait_group 1 keeps one batch queued behind the running one, so the tensor pipe
+// is not drained at k-block boundaries; the barrier after it only frees the stage of k-block i - 1 for reuse.
 //
 // CTA = 256 threads = 2 warpgroups; a tile is 128 x BN (each warpgroup owns 64 rows: one m64nBNk8 wgmma per product and k-step).
-//   BN = 128, BK = 32 (default): 2 x 64 KB of shared memory;   BN = 256, BK = 16 (phc_gemm_tc5s_set_tile(256)): 2 x 48 KB.
+//   BN = 128, BK = 32 (default): 3 x 64 KB of shared memory;   BN = 256, BK = 16 (phc_gemm_tc5s_set_tile(256)): 3 x 48 KB.
 // One launch takes up to PHC_GEMM_GROUP_MAX independent problems (the same layer of actor, critic and discriminator; dW and dX
 // of one layer): their tiles form one list walked by one persistent CTA per SM, in static striding or drawn from a global
 // counter (dynamic, the default: a CTA that got long tiles draws fewer of them).
@@ -45,7 +47,8 @@ struct Cfg {
   static constexpr int A_TILE = BM * BK * 4;
   static constexpr int B_TILE = BN * BK * 4;
   static constexpr int STAGE = 2 * (A_TILE + B_TILE);           // [A hi | A lo | B hi | B lo]
-  static constexpr int SMEM = 2 * STAGE;
+  static constexpr int STAGES = 3;
+  static constexpr int SMEM = STAGES * STAGE;
   static constexpr int SBO = BK * 32;                           // bytes between 8-row groups
   static constexpr int A_PER = BM * BK / NUM_THREADS;           // staged elements per thread
   static constexpr int B_PER = BN * BK / NUM_THREADS;
@@ -69,7 +72,6 @@ struct Params {
   Prob p[MAX_PROBLEMS];
   int count, total_tiles;
   unsigned int* sched;  // dynamic tile scheduler: {next tile, CTAs done} in global memory (both zero between launches); NULL = static striding
-  int single_pass;      // 1: one tensor-core product per fp32 product (plain TF32, ~1e-3 relative): no lo terms
 };
 
 __device__ __forceinline__ void wgmma_tf32_n128(float (&d)[64], uint64_t da, uint64_t db) {
@@ -89,7 +91,8 @@ __device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t da, ui
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
 __device__ __forceinline__ void wgmma_commit() { asm volatile("wgmma.commit_group.sync.aligned;" ::: "memory"); }
-__device__ __forceinline__ void wgmma_wait_all() { asm volatile("wgmma.wait_group.sync.aligned 0;" ::: "memory"); }
+template <int N>
+__device__ __forceinline__ void wgmma_wait() { asm volatile("wgmma.wait_group.sync.aligned %0;" ::"n"(N) : "memory"); }
 
 // shared-memory matrix descriptor (sm_90 GMMA): start address, LBO, SBO in 16-byte units, layout type 0 (no swizzle)
 __device__ __forceinline__ uint64_t smem_desc(uint32_t addr, uint32_t lbo, uint32_t sbo) {
@@ -113,49 +116,52 @@ __device__ __forceinline__ void sts128(uint32_t addr, float a, float b, float c,
 }
 __device__ __forceinline__ void sts32(uint32_t addr, float a) { asm volatile("st.shared.f32 [%0], %1;" ::"r"(addr), "f"(a) : "memory"); }
 
-// Element (r, k) of an R x BK operand tile, for staged element i of thread tid.
-//   k-contiguous: 16-byte chunk c = tid + i/4 * 256 holds (r, 4 kc .. 4 kc + 3) and lands at byte c * 16 of the tile (lanes of a
-//                 warp write 512 contiguous bytes);
-//   mn-contiguous: a warp gathers 8 rows x 4 k (32-byte global segments) and writes 32 distinct banks.
+// Where the 16-byte chunks of an R x BK operand tile come from and go to.  Thread tid stages chunks c = tid + i * 256.
+//   k-contiguous: chunk c holds (r, 4 kc .. 4 kc + 3) and lands at byte c * 16 of the tile (lanes of a warp write 512 contiguous
+//                 bytes);
+//   mn-contiguous: chunk c holds (r .. r + 3, k) with kl = c & 3, rl = (c >> 2) & 7, r = 4 (8 rh + rl), k = 4 kh + kl: a warp reads
+//                 128 contiguous bytes of each of 4 k-rows.  Element e of the chunk goes to byte off + 16 e = off ^ (e << 4) of the
+//                 tile, off = (r / 8) SBO + kh 128 + (rl & 1) 64 + kl 4 (bits 4-5 of off are zero), by a 4-byte store each.
+//                 SBO and 128 are multiples of the 32 banks' 128 bytes, so the bank of element e is 16 (rl & 1) + 4 e + kl; the
+//                 j-th store of a thread writes element e = j ^ (rl >> 1), so in each store the 32 lanes (kl, rl) write 32 distinct
+//                 banks.
 template <int R, int BK>
 struct Map {
   static constexpr int KC = BK / 4;
   __device__ static void kmaj(int c, int& r, int& kc) { r = (c & 7) + 8 * (c / (8 * KC)); kc = (c >> 3) % KC; }
-  __device__ static void mnmaj(int e, int& r, int& k, uint32_t& off) {
-    const int rl = e & 7, kl = (e >> 3) & 3, e2 = e >> 5, rh = e2 % (R / 8), kh = e2 / (R / 8);
-    r = rh * 8 + rl; k = kh * 4 + kl;
-    off = (uint32_t)(rh * BK * 32 + kh * 128 + rl * 16 + kl * 4);
+  __device__ static void mnmaj(int c, int& r, int& k, uint32_t& off) {
+    const int kl = c & 3, rl = (c >> 2) & 7, c2 = c >> 5, rh = c2 % (R / 32), kh = c2 / (R / 32);
+    r = 4 * (8 * rh + rl); k = 4 * kh + kl;
+    off = (uint32_t)((4 * rh + (rl >> 1)) * BK * 32 + kh * 128 + (rl & 1) * 64 + kl * 4);
   }
 };
 
-// global -> registers: PER elements of the R x BK tile at (r0, k0), zero outside [0, rows) x [0, K)
+// global -> registers: PER elements (PER / 4 chunks) of the R x BK tile at (r0, k0), zero outside [0, rows) x [0, K)
 template <int R, int BK, int PER>
 __device__ __forceinline__ void load_op(float (&v)[PER], const float* __restrict__ g, long long ld, bool kmaj, int r0, int rows, int k0,
                                         int K, int tid) {
   using Mp = Map<R, BK>;
-  if (kmaj) {
 #pragma unroll
-    for (int i = 0; i < PER / 4; ++i) {
-      int r, kc;
+  for (int i = 0; i < PER / 4; ++i) {
+    int r, k;                                                // the chunk's first element; its 4 elements are contiguous in g
+    const float* src;
+    if (kmaj) {
+      int kc;
       Mp::kmaj(tid + i * NUM_THREADS, r, kc);
-      const int rr = r0 + r, kk = k0 + 4 * kc;
-      const float* src = g + (long long)rr * ld + kk;
-      if (rr < rows && kk + 3 < K) {
-        const float4 t = *reinterpret_cast<const float4*>(src);
-        v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
-      } else {
-#pragma unroll
-        for (int e = 0; e < 4; ++e) v[4 * i + e] = (rr < rows && kk + e < K) ? src[e] : 0.f;
-      }
-    }
-  } else {
-#pragma unroll
-    for (int i = 0; i < PER; ++i) {
-      int r, k;
+      r += r0; k = k0 + 4 * kc;
+      src = g + (long long)r * ld + k;
+    } else {
       uint32_t off;
       Mp::mnmaj(tid + i * NUM_THREADS, r, k, off);
-      const int rr = r0 + r, kk = k0 + k;
-      v[i] = (rr < rows && kk < K) ? g[(long long)kk * ld + rr] : 0.f;
+      r += r0; k += k0;
+      src = g + (long long)k * ld + r;
+    }
+    if (kmaj ? (r < rows && k + 3 < K) : (r + 3 < rows && k < K)) {
+      const float4 t = *reinterpret_cast<const float4*>(src);
+      v[4 * i] = t.x; v[4 * i + 1] = t.y; v[4 * i + 2] = t.z; v[4 * i + 3] = t.w;
+    } else {
+#pragma unroll
+      for (int e = 0; e < 4; ++e) v[4 * i + e] = (kmaj ? (r < rows && k + e < K) : (r + e < rows && k < K)) ? src[e] : 0.f;
     }
   }
 }
@@ -174,14 +180,29 @@ __device__ __forceinline__ void store_op(const float (&v)[PER], const float (&w)
       if (MODE == 2) sts128(s_lo + off, w[4 * i], w[4 * i + 1], w[4 * i + 2], w[4 * i + 3]);
     }
   } else {
+    const int p = (tid >> 3) & 3;                            // rl >> 1 of every chunk of this thread
+    // u[j] = x[j ^ p]: the element the j-th store writes
+    auto perm = [p](const float* x, float (&u)[4]) {
+      u[0] = x[0]; u[1] = x[1]; u[2] = x[2]; u[3] = x[3];
+      if (p & 1) { const float t0 = u[0], t2 = u[2]; u[0] = u[1]; u[1] = t0; u[2] = u[3]; u[3] = t2; }
+      if (p & 2) { const float t0 = u[0], t1 = u[1]; u[0] = u[2]; u[1] = u[3]; u[2] = t0; u[3] = t1; }
+    };
 #pragma unroll
-    for (int i = 0; i < PER; ++i) {
+    for (int i = 0; i < PER / 4; ++i) {
       int r, k;
       uint32_t off;
       Mp::mnmaj(tid + i * NUM_THREADS, r, k, off);
-      sts32(s_hi + off, hi(v[i]));
-      if (MODE == 0) sts32(s_lo + off, split_lo(v[i]));
-      if (MODE == 2) sts32(s_lo + off, w[i]);
+      off ^= (uint32_t)p << 4;
+      float u[4], ul[4];
+      perm(&v[4 * i], u);
+      if (MODE == 2) perm(&w[4 * i], ul);
+#pragma unroll
+      for (int j = 0; j < 4; ++j) {
+        const uint32_t o = off ^ ((uint32_t)j << 4);
+        sts32(s_hi + o, hi(u[j]));
+        if (MODE == 0) sts32(s_lo + o, split_lo(u[j]));
+        if (MODE == 2) sts32(s_lo + o, ul[j]);
+      }
     }
   }
 }
@@ -194,16 +215,18 @@ __device__ __forceinline__ void split_rna(float x, float& h, float& l) {
   h = __uint_as_float(a); l = __uint_as_float(b);
 }
 
-template <int BN, bool PRESPLIT>
+// SINGLE: one tensor-core product per fp32 product (plain TF32, ~1e-3 relative): no lo terms
+template <int BN, bool PRESPLIT, bool SINGLE>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Params P) {
+  static_assert(!(PRESPLIT && SINGLE), "the pre-split operands are for the 3xTF32 products");
   using C = Cfg<BN>;
   constexpr int BK = C::BK;
+  constexpr int MODE = SINGLE ? 1 : PRESPLIT ? 2 : 0;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ int s_tile;
   const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, wq = (tid >> 5) & 3;
   const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
   const bool dyn = P.sched != nullptr;
-  const bool single = !PRESPLIT && P.single_pass != 0;
 
   for (int it = 0;; ++it) {
     int t;
@@ -231,38 +254,32 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
     float acc[BN / 2];
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
-    float va[C::A_PER], vb[C::B_PER], wa[PRESPLIT ? C::A_PER : 1], wb[PRESPLIT ? C::B_PER : 1];
-    constexpr int MODE = PRESPLIT ? 2 : 0;
-    auto load = [&](int kb) {
-      const int k0 = kb * BK;
-      load_op<BM, BK>(va, q.A, q.lda, ak, m0, q.M, k0, q.K, tid);
-      load_op<BN, BK>(vb, q.B, q.ldb, bk, n0, q.N, k0, q.K, tid);
+    // k-block j is staged through the registers v and shared-memory stage j % 3
+    struct Regs { float a[C::A_PER], b[C::B_PER], a_lo[PRESPLIT ? C::A_PER : 1], b_lo[PRESPLIT ? C::B_PER : 1]; };
+    Regs v;
+    auto load = [&](int j) {
+      const int k0 = (kb_begin + j) * BK;
+      load_op<BM, BK>(v.a, q.A, q.lda, ak, m0, q.M, k0, q.K, tid);
+      load_op<BN, BK>(v.b, q.B, q.ldb, bk, n0, q.N, k0, q.K, tid);
       if constexpr (PRESPLIT) {
-        load_op<BM, BK>(wa, q.A_lo, q.lda, ak, m0, q.M, k0, q.K, tid);
-        load_op<BN, BK>(wb, q.B_lo, q.ldb, bk, n0, q.N, k0, q.K, tid);
+        load_op<BM, BK>(v.a_lo, q.A_lo, q.lda, ak, m0, q.M, k0, q.K, tid);
+        load_op<BN, BK>(v.b_lo, q.B_lo, q.ldb, bk, n0, q.N, k0, q.K, tid);
       }
     };
-    auto store = [&](int buf) {
-      const uint32_t s = sbase + (uint32_t)(buf * C::STAGE);
-      if (single) {
-        store_op<BM, BK, C::A_PER, 1>(va, va, s, 0, ak, tid);
-        store_op<BN, BK, C::B_PER, 1>(vb, vb, s + 2 * C::A_TILE, 0, bk, tid);
-      } else if constexpr (PRESPLIT) {
-        store_op<BM, BK, C::A_PER, 2>(va, wa, s, s + C::A_TILE, ak, tid);
-        store_op<BN, BK, C::B_PER, 2>(vb, wb, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
+    auto stage = [&](int j) { return sbase + (uint32_t)((j % C::STAGES) * C::STAGE); };
+    auto store = [&](int j) {
+      const uint32_t s = stage(j);
+      if constexpr (PRESPLIT) {
+        store_op<BM, BK, C::A_PER, MODE>(v.a, v.a_lo, s, s + C::A_TILE, ak, tid);
+        store_op<BN, BK, C::B_PER, MODE>(v.b, v.b_lo, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
       } else {
-        store_op<BM, BK, C::A_PER, MODE>(va, va, s, s + C::A_TILE, ak, tid);
-        store_op<BN, BK, C::B_PER, MODE>(vb, vb, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
+        store_op<BM, BK, C::A_PER, MODE>(v.a, v.a, s, s + C::A_TILE, ak, tid);
+        store_op<BN, BK, C::B_PER, MODE>(v.b, v.b, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
       }
       fence_async_smem();                                   // generic-proxy writes -> visible to the tensor core's reads
     };
-
-    load(kb_begin);
-    store(0);
-    __syncthreads();
-#pragma unroll 1
-    for (int i = 0; i < nkb; ++i) {
-      const uint32_t s = sbase + (uint32_t)((i & 1) * C::STAGE);
+    auto mma = [&](int j) {                                  // one wgmma batch: every product of k-block j
+      const uint32_t s = stage(j);
       const uint32_t a_hi = s + (uint32_t)(wgi * 8 * C::SBO), a_lo = a_hi + C::A_TILE;
       const uint32_t b_hi = s + 2 * C::A_TILE, b_lo = b_hi + C::B_TILE;
       wgmma_fence();
@@ -270,20 +287,35 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
       for (int kk = 0; kk < BK / 8; ++kk) {
         const uint32_t o = (uint32_t)kk * 256u;
         const uint64_t dAh = smem_desc(a_hi + o, 128, C::SBO), dBh = smem_desc(b_hi + o, 128, C::SBO);
-        if (!single) {
+        if constexpr (!SINGLE) {
           wgmma_tf32<BN>(acc, smem_desc(a_lo + o, 128, C::SBO), dBh);
           wgmma_tf32<BN>(acc, dAh, smem_desc(b_lo + o, 128, C::SBO));
         }
         wgmma_tf32<BN>(acc, dAh, dBh);
       }
       wgmma_commit();
-      if (i + 1 < nkb) {                                     // next k-block into the other buffer while the wgmmas run
-        load(kb_begin + i + 1);
-        store((i + 1) & 1);
-      }
-      wgmma_wait_all();
+    };
+    // Step j: k-block j's wgmmas go out; k-block j + 1, loaded during step j - 1, is split and stored into the stage of
+    // j - 2, whose wgmmas the barrier of step j - 1 saw finish; then the loads of j + 2 are issued.  They come after the store
+    // on purpose: fence.proxy.async is a MEMBAR.CTA that waits for every memory access the thread has in flight, global loads
+    // included, so loads issued before it would be waited for right there -- which is also why a second register set would
+    // not let them start earlier.  Issued after it, they stay in flight through wait_group 1 (which leaves j's batch running
+    // behind j - 1's) and the barrier, up to the store of step j + 1.  The barrier makes j + 1's stage visible to both
+    // warpgroups and tells them j - 1's stage is free.
+    load(0);
+    store(0);
+    if (nkb > 1) load(1);
+    __syncthreads();
+#pragma unroll 1
+    for (int j = 0; j < nkb; ++j) {
+      mma(j);
+      if (j + 1 < nkb) store(j + 1);
+      if (j + 2 < nkb) load(j + 2);
+      wgmma_wait<1>();
       __syncthreads();
     }
+    wgmma_wait<0>();
+    __syncthreads();                                         // both warpgroups' last batch is done before its stage is refilled
 
     const bool ordered = q.turn != nullptr;                 // split-K slice: wait until the slices before it have added into C
     volatile unsigned int* turn = ordered ? q.turn + mi * q.tiles_n + ni : nullptr;
@@ -425,8 +457,23 @@ static int add_problem(Params& P, int n, int tiles, int bn, const float* A, cons
   return q.tile_count;
 }
 
+template <int BN, bool PRESPLIT, bool SINGLE>
+static int launch_kernel(const Params& P, cudaStream_t stream) {
+  static bool smem_set = false;
+  if (!smem_set) {
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, PRESPLIT, SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
+    if (e != cudaSuccess) return phc_check_cuda(e, "cudaFuncSetAttribute(gemm_wgmma)");
+    smem_set = true;
+  }
+  const int sms = num_sms();
+  const unsigned grid = (unsigned)(P.total_tiles < sms ? P.total_tiles : sms);
+  gemm_wgmma_kernel<BN, PRESPLIT, SINGLE><<<grid, NUM_THREADS, Cfg<BN>::SMEM, stream>>>(P);
+  phc_count_launches(1);
+  return phc_check_cuda(cudaGetLastError(), "gemm_wgmma_kernel launch");
+}
+
 template <int BN, bool PRESPLIT>
-static int launch(Params& P, bool dynamic_sched, cudaStream_t stream) {
+static int launch(Params& P, bool dynamic_sched, bool single, cudaStream_t stream) {
   // ordered problems: split-K, or accumulating into the same C as another problem of the launch (which then shares its turnstile)
   int owner[MAX_PROBLEMS];
   bool ordered = false;
@@ -488,17 +535,8 @@ static int launch(Params& P, bool dynamic_sched, cudaStream_t stream) {
     }
     P.sched = base + 2 * (launch_no++ % SCHED_SLOTS);
   }
-  static bool smem_set = false;
-  if (!smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, PRESPLIT>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
-    if (e != cudaSuccess) return phc_check_cuda(e, "cudaFuncSetAttribute(gemm_wgmma)");
-    smem_set = true;
-  }
-  const int sms = num_sms();
-  const unsigned grid = (unsigned)(P.total_tiles < sms ? P.total_tiles : sms);
-  gemm_wgmma_kernel<BN, PRESPLIT><<<grid, NUM_THREADS, Cfg<BN>::SMEM, stream>>>(P);
-  phc_count_launches(1);
-  return phc_check_cuda(cudaGetLastError(), "gemm_wgmma_kernel launch");
+  if constexpr (PRESPLIT) return launch_kernel<BN, true, false>(P, stream);
+  return single ? launch_kernel<BN, false, true>(P, stream) : launch_kernel<BN, false, false>(P, stream);
 }
 
 }  // namespace wg
@@ -565,9 +603,10 @@ extern "C" int phc_gemm_group(const PhcGemmDesc* d, int32_t count, void* stream)
     ++n;
   }
   if (n == 0) return PHC_OK;
-  P.count = n; P.total_tiles = tiles; P.single_pass = g_single_pass;
+  P.count = n; P.total_tiles = tiles;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
-  return bn == 256 ? launch<256, false>(P, g_sched == 1, st) : launch<128, false>(P, g_sched == 1, st);
+  const bool single = g_single_pass != 0;
+  return bn == 256 ? launch<256, false>(P, g_sched == 1, single, st) : launch<128, false>(P, g_sched == 1, single, st);
 }
 
 extern "C" int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, const float* B, int64_t ldb, int32_t b_kmajor, float* C,
@@ -600,7 +639,7 @@ extern "C" int phc_gemm_tc5(const float* A_hi, const float* A_lo, int64_t lda, i
   P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, lda, a_kmajor, B_hi, B_lo, ldb, b_kmajor, C, C_hi, C_lo, ldc, M, N, K, alpha, bias,
                               relu, mask, ldmask, accumulate, k_splits);
   P.count = 1;
-  return launch<128, true>(P, false, static_cast<cudaStream_t>(stream));
+  return launch<128, true>(P, false, false, static_cast<cudaStream_t>(stream));
 }
 
 extern "C" int phc_split_tf32(const float* x, int64_t ldx, int64_t rows, int32_t cols, float* hi, float* lo, int64_t ldo,
