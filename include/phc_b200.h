@@ -452,7 +452,24 @@ typedef struct PhcGemmDesc {
   int32_t accumulate, k_splits;
   const float* B_lo;        /* optional: the 3xTF32 low part of B, same layout and ldb, made by phc_split_lo; validated and not
                              * read (the kernel makes the identical low part from the tiles it stages) */
+  const float* B_img;       /* optional: B's weight image for this problem's N and K (phc_gemm_make_images), 16-byte aligned, with
+                             * a_kmajor only.  With 128 x 128 tiles the kernel then reads B from the image (one bulk copy per
+                             * k-block) and A straight into the tensor-core registers instead of staging both; the result is the
+                             * same bit for bit.  128 x 256 tiles and PHC_GEMM_TF32_SINGLE_PASS ignore it.  The image must be
+                             * remade whenever B changes. */
 } PhcGemmDesc;
+/* Weight image of a B operand (B(n,k) as in PhcGemmDesc, N x K): one block of 8192 floats per (128-row n-tile nt, 32-wide k-block
+ * kb), block nt * ceil(K / 32) + kb, each block [hi | lo] of 4096 floats with hi = trunc_tf32(B), lo = rna_tf32(B - hi) (the
+ * split the GEMM makes itself); inside a half, element (n, k) of the tile sits at float 256 (n / 8) + 32 (k / 4) + 4 (n % 8) + k % 4
+ * (8-row x 16-byte core matrices, K-major, no swizzle).  Zero outside N x K.  phc_gemm_image_floats(N, K) is its size.
+ * phc_gemm_make_images writes `count` images in one launch (more than 64 take one launch per 64). */
+typedef struct PhcGemmImageDesc {
+  const float* B; int64_t ldb; int32_t b_kmajor;
+  int32_t N, K;
+  float* img;
+} PhcGemmImageDesc;
+PHC_API int64_t phc_gemm_image_floats(int32_t N, int32_t K);
+PHC_API int phc_gemm_make_images(const PhcGemmImageDesc* images, int32_t count, void* stream);
 /* lo[i] = rna_tf32(x[i] - trunc_tf32(x[i])): the second TF32 term of every fp32 value, what the GEMM computes per staged tile */
 PHC_API int phc_split_lo(const float* x, float* lo, int64_t n, void* stream);
 PHC_API int phc_gemm_group(const PhcGemmDesc* problems, int32_t count, void* stream);

@@ -82,7 +82,11 @@ class PhcGemmDesc(C.Structure):
     _fields_ = [("A", _p), ("lda", C.c_int64), ("a_kmajor", C.c_int32), ("B", _p), ("ldb", C.c_int64), ("b_kmajor", C.c_int32),
                 ("C", _p), ("ldc", C.c_int64), ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("alpha", C.c_float),
                 ("bias", _p), ("act", C.c_int32), ("aux", _p), ("ldaux", C.c_int64), ("accumulate", C.c_int32), ("k_splits", C.c_int32),
-                ("B_lo", _p)]
+                ("B_lo", _p), ("B_img", _p)]
+
+
+class PhcGemmImageDesc(C.Structure):
+    _fields_ = [("B", _p), ("ldb", C.c_int64), ("b_kmajor", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("img", _p)]
 
 
 class PhcColsumDesc(C.Structure):
@@ -137,6 +141,8 @@ SIGNATURES = {
                                C.c_int32, C.c_float, _p, C.c_int32, _p, C.c_int64, C.c_int32, C.c_int32, _p]),
     "phc_gemm_group": (C.c_int, [C.POINTER(PhcGemmDesc), C.c_int32, _p]),
     "phc_split_lo": (C.c_int, [_p, _p, C.c_int64, _p]),
+    "phc_gemm_image_floats": (C.c_int64, [C.c_int32, C.c_int32]),
+    "phc_gemm_make_images": (C.c_int, [C.POINTER(PhcGemmImageDesc), C.c_int32, _p]),
     "phc_gemm_tc5s": (C.c_int, [_p, C.c_int64, C.c_int32, _p, C.c_int64, C.c_int32, _p, C.c_int64, C.c_int32, C.c_int32,
                                 C.c_int32, C.c_float, _p, C.c_int32, _p, C.c_int64, C.c_int32, C.c_int32, _p]),
     "phc_gemm_tc5s_set_ctas": (C.c_int, [C.c_int32]),

@@ -24,10 +24,14 @@
 // result does not depend on which CTA finishes first, so a run is reproducible bit for bit.  A launch with ordered problems always
 // draws its tiles dynamically; a slice then only waits for a lower-numbered tile that a running CTA has already drawn.
 // phc_gemm_tc5 is the same kernel with operands pre-split in global memory (hi / lo arrays loaded instead of split).
+// A 3xTF32 problem with 128 x 128 tiles that comes with a weight image of B (PhcGemmDesc.B_img) skips the staging: B arrives
+// pre-split by bulk copy and A goes from global memory straight into the wgmma register fragment (the image loop below).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
 #include <string.h>
+
+#include <type_traits>
 
 #include "../../include/phc_b200.h"
 #include "phc_common.cuh"
@@ -54,8 +58,16 @@ struct Cfg {
   static constexpr int B_PER = BN * BK / NUM_THREADS;
 };
 
+// Weight images (PhcGemmDesc.B_img, made by phc_gemm_make_images): B pre-split and pre-laid-out for the 128 x 128 x 32 tile.
+// One block of IMG_BLOCK floats per (128-row n-tile, 32-wide k-block), block (nt, kb) at nt * ceil(K / 32) + kb; each block is
+// [hi | lo], every half a 128 x 32 tile in the no-swizzle K-major layout the staged loop writes, zero outside N x K.  A stage of B
+// is then one bulk copy, and A goes to wgmma from registers (see the image loop in gemm_wgmma_kernel).
+constexpr int IMG_ROWS = 128, IMG_BK = 32, IMG_HALF = IMG_ROWS * IMG_BK, IMG_BLOCK = 2 * IMG_HALF;
+constexpr int IMG_STAGES = 4;             // B ring of the image loop: 4 x 32 KB, inside the staged loop's 3 x 64 KB
+
 struct Prob {
   const float* A; const float* B; const float* A_lo; const float* B_lo;      // A_lo / B_lo: pre-split operands (phc_gemm_tc5)
+  const float* B_img;                                                          // weight image of B (128 x 128 tiles only), or NULL
   float* C; float* C_hi; float* C_lo;                                          // C_hi / C_lo: split copies of the result (phc_gemm_tc5)
   const float* bias;
   float* aux;
@@ -87,6 +99,45 @@ __device__ __forceinline__ void wgmma_tf32_n256(float (&d)[128], uint64_t da, ui
       "wgmma.mma_async.sync.aligned.m64n256k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63, %64, %65, %66, %67, %68, %69, %70, %71, %72, %73, %74, %75, %76, %77, %78, %79, %80, %81, %82, %83, %84, %85, %86, %87, %88, %89, %90, %91, %92, %93, %94, %95, %96, %97, %98, %99, %100, %101, %102, %103, %104, %105, %106, %107, %108, %109, %110, %111, %112, %113, %114, %115, %116, %117, %118, %119, %120, %121, %122, %123, %124, %125, %126, %127}, %128, %129, p, 1, 1;\n\t}"
       : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63]), "+f"(d[64]), "+f"(d[65]), "+f"(d[66]), "+f"(d[67]), "+f"(d[68]), "+f"(d[69]), "+f"(d[70]), "+f"(d[71]), "+f"(d[72]), "+f"(d[73]), "+f"(d[74]), "+f"(d[75]), "+f"(d[76]), "+f"(d[77]), "+f"(d[78]), "+f"(d[79]), "+f"(d[80]), "+f"(d[81]), "+f"(d[82]), "+f"(d[83]), "+f"(d[84]), "+f"(d[85]), "+f"(d[86]), "+f"(d[87]), "+f"(d[88]), "+f"(d[89]), "+f"(d[90]), "+f"(d[91]), "+f"(d[92]), "+f"(d[93]), "+f"(d[94]), "+f"(d[95]), "+f"(d[96]), "+f"(d[97]), "+f"(d[98]), "+f"(d[99]), "+f"(d[100]), "+f"(d[101]), "+f"(d[102]), "+f"(d[103]), "+f"(d[104]), "+f"(d[105]), "+f"(d[106]), "+f"(d[107]), "+f"(d[108]), "+f"(d[109]), "+f"(d[110]), "+f"(d[111]), "+f"(d[112]), "+f"(d[113]), "+f"(d[114]), "+f"(d[115]), "+f"(d[116]), "+f"(d[117]), "+f"(d[118]), "+f"(d[119]), "+f"(d[120]), "+f"(d[121]), "+f"(d[122]), "+f"(d[123]), "+f"(d[124]), "+f"(d[125]), "+f"(d[126]), "+f"(d[127])
       : "l"(da), "l"(db));
+}
+
+// the same product with A from registers: a[0..3] is the warp's 16 x 8 tf32 fragment, (row lane / 4 + 8 (i & 1), col lane % 4 + 4 (i >> 1))
+__device__ __forceinline__ void wgmma_tf32_n128_rs(float (&d)[64], const uint32_t (&a)[4], uint64_t db) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\tsetp.ne.b32 p, 1, 0;\n\t"
+      "wgmma.mma_async.sync.aligned.m64n128k8.f32.tf32.tf32 {%0, %1, %2, %3, %4, %5, %6, %7, %8, %9, %10, %11, %12, %13, %14, %15, %16, %17, %18, %19, %20, %21, %22, %23, %24, %25, %26, %27, %28, %29, %30, %31, %32, %33, %34, %35, %36, %37, %38, %39, %40, %41, %42, %43, %44, %45, %46, %47, %48, %49, %50, %51, %52, %53, %54, %55, %56, %57, %58, %59, %60, %61, %62, %63}, {%64, %65, %66, %67}, %68, p, 1, 1;\n\t}"
+      : "+f"(d[0]), "+f"(d[1]), "+f"(d[2]), "+f"(d[3]), "+f"(d[4]), "+f"(d[5]), "+f"(d[6]), "+f"(d[7]), "+f"(d[8]), "+f"(d[9]), "+f"(d[10]), "+f"(d[11]), "+f"(d[12]), "+f"(d[13]), "+f"(d[14]), "+f"(d[15]), "+f"(d[16]), "+f"(d[17]), "+f"(d[18]), "+f"(d[19]), "+f"(d[20]), "+f"(d[21]), "+f"(d[22]), "+f"(d[23]), "+f"(d[24]), "+f"(d[25]), "+f"(d[26]), "+f"(d[27]), "+f"(d[28]), "+f"(d[29]), "+f"(d[30]), "+f"(d[31]), "+f"(d[32]), "+f"(d[33]), "+f"(d[34]), "+f"(d[35]), "+f"(d[36]), "+f"(d[37]), "+f"(d[38]), "+f"(d[39]), "+f"(d[40]), "+f"(d[41]), "+f"(d[42]), "+f"(d[43]), "+f"(d[44]), "+f"(d[45]), "+f"(d[46]), "+f"(d[47]), "+f"(d[48]), "+f"(d[49]), "+f"(d[50]), "+f"(d[51]), "+f"(d[52]), "+f"(d[53]), "+f"(d[54]), "+f"(d[55]), "+f"(d[56]), "+f"(d[57]), "+f"(d[58]), "+f"(d[59]), "+f"(d[60]), "+f"(d[61]), "+f"(d[62]), "+f"(d[63])
+      : "r"(a[0]), "r"(a[1]), "r"(a[2]), "r"(a[3]), "l"(db));
+}
+
+// mbarrier + bulk copy (the B stages of the image loop; the CTA is its own cluster of one)
+__device__ __forceinline__ void mbar_init(uint32_t bar, uint32_t count) {
+  asm volatile("mbarrier.init.shared::cta.b64 [%0], %1;" ::"r"(bar), "r"(count) : "memory");
+}
+__device__ __forceinline__ void mbar_init_fence() { asm volatile("fence.mbarrier_init.release.cluster;" ::: "memory"); }
+__device__ __forceinline__ void mbar_expect_tx(uint32_t bar, uint32_t bytes) {
+  asm volatile("mbarrier.arrive.expect_tx.shared::cta.b64 _, [%0], %1;" ::"r"(bar), "r"(bytes) : "memory");
+}
+__device__ __forceinline__ void mbar_wait(uint32_t bar, uint32_t parity) {
+  asm volatile(
+      "{\n\t.reg .pred p;\n\t"
+      "WAIT:\n\t"
+      "mbarrier.try_wait.parity.shared::cta.b64 p, [%0], %1;\n\t"
+      "@!p bra WAIT;\n\t}" ::"r"(bar), "r"(parity) : "memory");
+}
+__device__ __forceinline__ void bulk_g2s(uint32_t dst, const void* src, uint32_t bytes, uint32_t bar) {
+  asm volatile("cp.async.bulk.shared::cluster.global.mbarrier::complete_tx::bytes [%0], [%1], %2, [%3];"
+               ::"r"(dst), "l"(src), "r"(bytes), "r"(bar) : "memory");
+}
+
+// pins register operands of the wgmma A fragment in place: computed before the wgmma.fence that precedes the batch, and kept
+// live up to the wait_group that retires it (the compiler would otherwise move the splits past the fence or reuse the registers)
+template <int N>
+__device__ __forceinline__ void reg_fence(uint32_t (&r)[N][4]) {
+#pragma unroll
+  for (int i = 0; i < N; ++i)
+#pragma unroll
+    for (int j = 0; j < 4; ++j) asm volatile("" : "+r"(r[i][j])::"memory");
 }
 
 __device__ __forceinline__ void wgmma_fence() { asm volatile("wgmma.fence.sync.aligned;" ::: "memory"); }
@@ -222,11 +273,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
   using C = Cfg<BN>;
   constexpr int BK = C::BK;
   constexpr int MODE = SINGLE ? 1 : PRESPLIT ? 2 : 0;
+  // single pass stays on the staged loop: ptxas serialises the wgmmas of its image loop (C7513)
+  constexpr bool HAS_IMG = BN == IMG_ROWS && BK == IMG_BK && !PRESPLIT && !SINGLE;
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ int s_tile;
+  __shared__ __align__(8) uint64_t s_bar[IMG_STAGES];      // one mbarrier per B stage of the image loop
   const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, wq = (tid >> 5) & 3;
   const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
+  const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(s_bar);
   const bool dyn = P.sched != nullptr;
+  int ring = 0;                                             // k-blocks the image loop has taken through its B ring so far
+  if constexpr (HAS_IMG) {
+    if (tid == 0) {
+#pragma unroll
+      for (int s = 0; s < IMG_STAGES; ++s) mbar_init(bar0 + 8 * s, 1);
+      mbar_init_fence();
+    }
+    __syncthreads();
+  }
 
   for (int it = 0;; ++it) {
     int t;
@@ -254,67 +318,152 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
     float acc[BN / 2];
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
-    // k-block j is staged through the registers v and shared-memory stage j % 3
-    struct Regs { float a[C::A_PER], b[C::B_PER], a_lo[PRESPLIT ? C::A_PER : 1], b_lo[PRESPLIT ? C::B_PER : 1]; };
-    Regs v;
-    auto load = [&](int j) {
-      const int k0 = (kb_begin + j) * BK;
-      load_op<BM, BK>(v.a, q.A, q.lda, ak, m0, q.M, k0, q.K, tid);
-      load_op<BN, BK>(v.b, q.B, q.ldb, bk, n0, q.N, k0, q.K, tid);
-      if constexpr (PRESPLIT) {
-        load_op<BM, BK>(v.a_lo, q.A_lo, q.lda, ak, m0, q.M, k0, q.K, tid);
-        load_op<BN, BK>(v.b_lo, q.B_lo, q.ldb, bk, n0, q.N, k0, q.K, tid);
-      }
-    };
-    auto stage = [&](int j) { return sbase + (uint32_t)((j % C::STAGES) * C::STAGE); };
-    auto store = [&](int j) {
-      const uint32_t s = stage(j);
-      if constexpr (PRESPLIT) {
-        store_op<BM, BK, C::A_PER, MODE>(v.a, v.a_lo, s, s + C::A_TILE, ak, tid);
-        store_op<BN, BK, C::B_PER, MODE>(v.b, v.b_lo, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
-      } else {
-        store_op<BM, BK, C::A_PER, MODE>(v.a, v.a, s, s + C::A_TILE, ak, tid);
-        store_op<BN, BK, C::B_PER, MODE>(v.b, v.b, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
-      }
-      fence_async_smem();                                   // generic-proxy writes -> visible to the tensor core's reads
-    };
-    auto mma = [&](int j) {                                  // one wgmma batch: every product of k-block j
-      const uint32_t s = stage(j);
-      const uint32_t a_hi = s + (uint32_t)(wgi * 8 * C::SBO), a_lo = a_hi + C::A_TILE;
-      const uint32_t b_hi = s + 2 * C::A_TILE, b_lo = b_hi + C::B_TILE;
-      wgmma_fence();
+    bool staged = true;
+    if constexpr (HAS_IMG) {
+      if (q.B_img != nullptr) {                              // (uniform) B from its weight image, A from registers
+        staged = false;
+        // B: k-block j arrives in ring slot (ring + j) % IMG_STAGES by one bulk copy that thread 0 issues, IMG_STAGES k-blocks
+        // ahead; the barrier after wait_group 1 of step j says that the slot of j - 1 is free again.  No generic-proxy write
+        // touches B, so there is no proxy fence.
+        // A: every thread loads its own part of the wgmma A fragment straight from global memory and splits it in registers:
+        // ar[4 kk + i] = A(r + 8 (i & 1), k0 + 8 kk + c + 4 (i >> 1)), r = the warp's row lane / 4, c = lane % 4.  The loads
+        // of k-block j + 1 are in flight during the wgmmas of j.  A batch behind wait_group 1 still reads its A registers,
+        // so there are two split sets, used alternately, and the loop is unrolled by two to keep their indices static.
+        // The products, their order per k8 and the k order are those of the staged loop: the results are the same bit for bit.
+        const int r = m0 + wgi * 64 + wq * 16 + (lane >> 2), c = lane & 3;
+        const bool ok0 = r < q.M, ok1 = r + 8 < q.M;
+        const float* arow0 = q.A + (long long)(ok0 ? r : 0) * q.lda + c;
+        const float* arow1 = q.A + (long long)(ok1 ? r + 8 : 0) * q.lda + c;
+        float ar[16];
+        auto load_a = [&](int j) {
+          const int k0 = (kb_begin + j) * BK;
+          const bool full = k0 + BK <= q.K;
 #pragma unroll
-      for (int kk = 0; kk < BK / 8; ++kk) {
-        const uint32_t o = (uint32_t)kk * 256u;
-        const uint64_t dAh = smem_desc(a_hi + o, 128, C::SBO), dBh = smem_desc(b_hi + o, 128, C::SBO);
-        if constexpr (!SINGLE) {
-          wgmma_tf32<BN>(acc, smem_desc(a_lo + o, 128, C::SBO), dBh);
-          wgmma_tf32<BN>(acc, dAh, smem_desc(b_lo + o, 128, C::SBO));
-        }
-        wgmma_tf32<BN>(acc, dAh, dBh);
-      }
-      wgmma_commit();
-    };
-    // Step j: k-block j's wgmmas go out; k-block j + 1, loaded during step j - 1, is split and stored into the stage of
-    // j - 2, whose wgmmas the barrier of step j - 1 saw finish; then the loads of j + 2 are issued.  They come after the store
-    // on purpose: fence.proxy.async is a MEMBAR.CTA that waits for every memory access the thread has in flight, global loads
-    // included, so loads issued before it would be waited for right there -- which is also why a second register set would
-    // not let them start earlier.  Issued after it, they stay in flight through wait_group 1 (which leaves j's batch running
-    // behind j - 1's) and the barrier, up to the store of step j + 1.  The barrier makes j + 1's stage visible to both
-    // warpgroups and tells them j - 1's stage is free.
-    load(0);
-    store(0);
-    if (nkb > 1) load(1);
-    __syncthreads();
+          for (int e = 0; e < 16; ++e) {
+            const int k = k0 + 8 * (e >> 2) + 4 * ((e >> 1) & 1);
+            const bool ok = ((e & 1) ? ok1 : ok0) && (full || k + c < q.K);
+            ar[e] = ok ? ((e & 1) ? arow1 : arow0)[k] : 0.f;
+          }
+        };
+        uint32_t ah[2][BK / 8][4], al[2][SINGLE ? 1 : BK / 8][4];
+        constexpr uint32_t B_BYTES = (SINGLE ? 1 : 2) * IMG_HALF * 4, SLOT = 2 * IMG_HALF * 4;
+        const float* img = q.B_img + (long long)ni * q.kb_total * IMG_BLOCK;
+        auto issue = [&](int j) {
+          const int s = (ring + j) % IMG_STAGES;
+          mbar_expect_tx(bar0 + 8 * s, B_BYTES);
+          bulk_g2s(sbase + s * SLOT, img + (long long)(kb_begin + j) * IMG_BLOCK, B_BYTES, bar0 + 8 * s);
+        };
+        if (tid == 0)
+          for (int j = 0; j < min(nkb, IMG_STAGES); ++j) issue(j);
+        load_a(0);
+        auto step = [&](int j, auto set) {
+          constexpr int S = decltype(set)::value;
+#pragma unroll
+          for (int e = 0; e < 16; ++e) {
+            ah[S][e >> 2][e & 3] = __float_as_uint(trunc_hi(ar[e]));
+            if constexpr (!SINGLE) al[S][e >> 2][e & 3] = __float_as_uint(split_lo(ar[e]));
+          }
+          if (j + 1 < nkb) load_a(j + 1);
+          const int s = (ring + j) % IMG_STAGES;
+          mbar_wait(bar0 + 8 * s, (uint32_t)((ring + j) / IMG_STAGES) & 1u);
+          uint64_t dB[BK / 8][2];                            // B descriptors (hi, lo) per k8, also made before the fence
+#pragma unroll
+          for (int kk = 0; kk < BK / 8; ++kk)
+#pragma unroll
+            for (int h = 0; h < 2; ++h) {
+              dB[kk][h] = smem_desc(sbase + s * SLOT + h * IMG_HALF * 4 + kk * 256, 128, C::SBO);
+              asm volatile("" : "+l"(dB[kk][h])::"memory");
+            }
+          reg_fence(ah[S]);
+          if constexpr (!SINGLE) reg_fence(al[S]);
+          wgmma_fence();
+#pragma unroll
+          for (int kk = 0; kk < BK / 8; ++kk) {
+            if constexpr (!SINGLE) {
+              wgmma_tf32_n128_rs(acc, al[S][kk], dB[kk][0]);
+              wgmma_tf32_n128_rs(acc, ah[S][kk], dB[kk][1]);
+            }
+            wgmma_tf32_n128_rs(acc, ah[S][kk], dB[kk][0]);
+          }
+          wgmma_commit();
+          wgmma_wait<1>();
+          reg_fence(ah[S ^ 1]);                                // the batch of j - 1 is done with its set
+          if constexpr (!SINGLE) reg_fence(al[S ^ 1]);
+          __syncthreads();
+          if (tid == 0 && j >= 1 && j - 1 + IMG_STAGES < nkb) issue(j - 1 + IMG_STAGES);
+        };
 #pragma unroll 1
-    for (int j = 0; j < nkb; ++j) {
-      mma(j);
-      if (j + 1 < nkb) store(j + 1);
-      if (j + 2 < nkb) load(j + 2);
-      wgmma_wait<1>();
-      __syncthreads();
+        for (int j = 0; j < nkb; j += 2) {
+          step(j, std::integral_constant<int, 0>());
+          if (j + 1 < nkb) step(j + 1, std::integral_constant<int, 1>());
+        }
+        wgmma_wait<0>();
+        ring += nkb;
+      }
     }
-    wgmma_wait<0>();
+    if (staged) {
+      // k-block j is staged through the registers v and shared-memory stage j % 3
+      struct Regs { float a[C::A_PER], b[C::B_PER], a_lo[PRESPLIT ? C::A_PER : 1], b_lo[PRESPLIT ? C::B_PER : 1]; };
+      Regs v;
+      auto load = [&](int j) {
+        const int k0 = (kb_begin + j) * BK;
+        load_op<BM, BK>(v.a, q.A, q.lda, ak, m0, q.M, k0, q.K, tid);
+        load_op<BN, BK>(v.b, q.B, q.ldb, bk, n0, q.N, k0, q.K, tid);
+        if constexpr (PRESPLIT) {
+          load_op<BM, BK>(v.a_lo, q.A_lo, q.lda, ak, m0, q.M, k0, q.K, tid);
+          load_op<BN, BK>(v.b_lo, q.B_lo, q.ldb, bk, n0, q.N, k0, q.K, tid);
+        }
+      };
+      auto stage = [&](int j) { return sbase + (uint32_t)((j % C::STAGES) * C::STAGE); };
+      auto store = [&](int j) {
+        const uint32_t s = stage(j);
+        if constexpr (PRESPLIT) {
+          store_op<BM, BK, C::A_PER, MODE>(v.a, v.a_lo, s, s + C::A_TILE, ak, tid);
+          store_op<BN, BK, C::B_PER, MODE>(v.b, v.b_lo, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
+        } else {
+          store_op<BM, BK, C::A_PER, MODE>(v.a, v.a, s, s + C::A_TILE, ak, tid);
+          store_op<BN, BK, C::B_PER, MODE>(v.b, v.b, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
+        }
+        fence_async_smem();                                   // generic-proxy writes -> visible to the tensor core's reads
+      };
+      auto mma = [&](int j) {                                  // one wgmma batch: every product of k-block j
+        const uint32_t s = stage(j);
+        const uint32_t a_hi = s + (uint32_t)(wgi * 8 * C::SBO), a_lo = a_hi + C::A_TILE;
+        const uint32_t b_hi = s + 2 * C::A_TILE, b_lo = b_hi + C::B_TILE;
+        wgmma_fence();
+  #pragma unroll
+        for (int kk = 0; kk < BK / 8; ++kk) {
+          const uint32_t o = (uint32_t)kk * 256u;
+          const uint64_t dAh = smem_desc(a_hi + o, 128, C::SBO), dBh = smem_desc(b_hi + o, 128, C::SBO);
+          if constexpr (!SINGLE) {
+            wgmma_tf32<BN>(acc, smem_desc(a_lo + o, 128, C::SBO), dBh);
+            wgmma_tf32<BN>(acc, dAh, smem_desc(b_lo + o, 128, C::SBO));
+          }
+          wgmma_tf32<BN>(acc, dAh, dBh);
+        }
+        wgmma_commit();
+      };
+      // Step j: k-block j's wgmmas go out; k-block j + 1, loaded during step j - 1, is split and stored into the stage of
+      // j - 2, whose wgmmas the barrier of step j - 1 saw finish; then the loads of j + 2 are issued.  They come after the store
+      // on purpose: fence.proxy.async is a MEMBAR.CTA that waits for every memory access the thread has in flight, global loads
+      // included, so loads issued before it would be waited for right there -- which is also why a second register set would
+      // not let them start earlier.  Issued after it, they stay in flight through wait_group 1 (which leaves j's batch running
+      // behind j - 1's) and the barrier, up to the store of step j + 1.  The barrier makes j + 1's stage visible to both
+      // warpgroups and tells them j - 1's stage is free.
+      load(0);
+      store(0);
+      if (nkb > 1) load(1);
+      __syncthreads();
+  #pragma unroll 1
+      for (int j = 0; j < nkb; ++j) {
+        mma(j);
+        if (j + 1 < nkb) store(j + 1);
+        if (j + 2 < nkb) load(j + 2);
+        wgmma_wait<1>();
+        __syncthreads();
+      }
+      wgmma_wait<0>();
+    }
     __syncthreads();                                         // both warpgroups' last batch is done before its stage is refilled
 
     const bool ordered = q.turn != nullptr;                 // split-K slice: wait until the slices before it have added into C
@@ -417,6 +566,40 @@ __global__ void split_tf32_kernel(const float* __restrict__ x, int64_t ldx, int6
   }
 }
 
+// Weight images: CTA b writes image block b of the launch, [hi | lo] of one 128 x 32 tile of B in the K-major layout of the
+// staged loop (16-byte chunk c = tid + 256 i holds (r, 4 kc .. 4 kc + 3), Map::kmaj), split by the kernel's own trunc_hi / split_lo
+constexpr int IMG_JOBS = 64;
+struct ImgJob { const float* B; long long ldb; float* img; long long block_begin; int b_k, N, K, kbs; };
+struct ImgParams { ImgJob j[IMG_JOBS]; int count; long long total_blocks; };
+
+__global__ void __launch_bounds__(NUM_THREADS) weight_image_kernel(const __grid_constant__ ImgParams P) {
+  using Mp = Map<IMG_ROWS, IMG_BK>;
+  for (long long b = blockIdx.x; b < P.total_blocks; b += gridDim.x) {
+    int i = 0;
+    while (i + 1 < P.count && b >= P.j[i + 1].block_begin) ++i;
+    const ImgJob& J = P.j[i];
+    const long long lb = b - J.block_begin;
+    const int n0 = (int)(lb / J.kbs) * IMG_ROWS, k0 = (int)(lb % J.kbs) * IMG_BK;
+    float4* hi = reinterpret_cast<float4*>(J.img + lb * IMG_BLOCK);
+    float4* lo = hi + IMG_HALF / 4;
+#pragma unroll
+    for (int it = 0; it < IMG_HALF / 4 / NUM_THREADS; ++it) {
+      const int c = threadIdx.x + it * NUM_THREADS;
+      int r, kc;
+      Mp::kmaj(c, r, kc);
+      const int n = n0 + r, k = k0 + 4 * kc;
+      float v[4];
+#pragma unroll
+      for (int e = 0; e < 4; ++e)
+        v[e] = (n < J.N && k + e < J.K) ? (J.b_k ? J.B[(long long)n * J.ldb + k + e] : J.B[(long long)(k + e) * J.ldb + n]) : 0.f;
+      hi[c] = make_float4(trunc_hi(v[0]), trunc_hi(v[1]), trunc_hi(v[2]), trunc_hi(v[3]));
+      lo[c] = make_float4(split_lo(v[0]), split_lo(v[1]), split_lo(v[2]), split_lo(v[3]));
+    }
+  }
+}
+
+static long long image_blocks(int N, int K) { return (long long)((N + IMG_ROWS - 1) / IMG_ROWS) * ((K + IMG_BK - 1) / IMG_BK); }
+
 static int g_single_pass = 0;
 static int g_tile = 0;        // 0: default (128), else the tile width 128 | 256
 static int g_sched = -1;      // -1: not decided yet (env PHC_TC5S_SCHED = static | dynamic; default dynamic), 0 static, 1 dynamic
@@ -436,11 +619,11 @@ static int num_sms() {
 
 // fills P.p[n] for one problem; returns the number of tiles it adds
 static int add_problem(Params& P, int n, int tiles, int bn, const float* A, const float* A_lo, long long lda, int a_k, const float* B,
-                       const float* B_lo, long long ldb, int b_k, float* Cm, float* C_hi, float* C_lo, long long ldc, int M, int N, int K,
+                       const float* B_lo, const float* B_img, long long ldb, int b_k, float* Cm, float* C_hi, float* C_lo, long long ldc, int M, int N, int K,
                        float alpha, const float* bias, int act, float* aux, long long ldaux, int accumulate, int k_splits) {
   const int bk = bn == 128 ? Cfg<128>::BK : Cfg<256>::BK;
   Prob& q = P.p[n];
-  q.A = A; q.A_lo = A_lo; q.B = B; q.B_lo = B_lo; q.C = Cm; q.C_hi = C_hi; q.C_lo = C_lo; q.bias = bias; q.aux = aux;
+  q.A = A; q.A_lo = A_lo; q.B = B; q.B_lo = B_lo; q.B_img = bn == IMG_ROWS ? B_img : nullptr; q.C = Cm; q.C_hi = C_hi; q.C_lo = C_lo; q.bias = bias; q.aux = aux;
   q.lda = lda; q.ldb = ldb; q.ldc = ldc; q.ldaux = ldaux; q.M = M; q.N = N; q.K = K; q.alpha = alpha; q.act = act;
   q.accumulate = accumulate ? 1 : 0; q.a_k = a_k ? 1 : 0; q.b_k = b_k ? 1 : 0;
   int ks = k_splits < 1 ? 1 : k_splits;
@@ -557,6 +740,7 @@ static int validate_group(const PhcGemmDesc* d, int32_t count) {
     if (g.act >= PHC_ACT_RELU_BITS && g.aux && ((reinterpret_cast<uintptr_t>(g.aux) & 3) || g.ldaux < (g.N + 31) / 32)) { phc_set_error("phc_gemm_group: bit-mask aux needs ldaux >= ceil(N / 32) words"); return PHC_ERR_INVALID_ARG; }
     if (ks > 1 && (!g.accumulate || g.act || g.aux)) { phc_set_error("phc_gemm_group: split-K needs accumulate=1 and a linear epilogue"); return PHC_ERR_INVALID_ARG; }
     if (g.B_lo && (reinterpret_cast<uintptr_t>(g.B_lo) & 15)) { phc_set_error("phc_gemm_group: B_lo must be 16-byte aligned"); return PHC_ERR_INVALID_ARG; }
+    if (g.B_img && ((reinterpret_cast<uintptr_t>(g.B_img) & 15) || !g.a_kmajor)) { phc_set_error("phc_gemm_group: B_img must be 16-byte aligned and comes with a_kmajor only"); return PHC_ERR_INVALID_ARG; }
   }
   // write hazards: the C spans [C, C + (M - 1) ldc + N) of two problems may only overlap when both accumulate into the same C with
   // the same shape -- they then share a turnstile and add in problem order; any other overlap would race (plain stores, or
@@ -598,7 +782,7 @@ extern "C" int phc_gemm_group(const PhcGemmDesc* d, int32_t count, void* stream)
   for (int i = 0; i < count; ++i) {
     const PhcGemmDesc& g = d[i];
     if (g.M == 0 || g.N == 0) continue;
-    tiles += add_problem(P, n, tiles, bn, g.A, nullptr, g.lda, g.a_kmajor, g.B, nullptr, g.ldb, g.b_kmajor, g.C, nullptr, nullptr, g.ldc,
+    tiles += add_problem(P, n, tiles, bn, g.A, nullptr, g.lda, g.a_kmajor, g.B, nullptr, g.B_img, g.ldb, g.b_kmajor, g.C, nullptr, nullptr, g.ldc,
                          g.M, g.N, g.K, g.alpha, g.bias, g.act, g.aux, g.ldaux, g.accumulate, g.k_splits);
     ++n;
   }
@@ -615,7 +799,7 @@ extern "C" int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, cons
   PhcGemmDesc d;
   d.A = A; d.lda = lda; d.a_kmajor = a_kmajor; d.B = B; d.ldb = ldb; d.b_kmajor = b_kmajor; d.C = C; d.ldc = ldc;
   d.M = M; d.N = N; d.K = K; d.alpha = alpha; d.bias = bias; d.act = act; d.aux = aux; d.ldaux = ldaux;
-  d.accumulate = accumulate; d.k_splits = k_splits; d.B_lo = nullptr;
+  d.accumulate = accumulate; d.k_splits = k_splits; d.B_lo = nullptr; d.B_img = nullptr;
   return phc_gemm_group(&d, 1, stream);
 }
 
@@ -636,7 +820,7 @@ extern "C" int phc_gemm_tc5(const float* A_hi, const float* A_lo, int64_t lda, i
   if ((C_hi == nullptr) != (C_lo == nullptr) || (C_hi && accumulate)) { phc_set_error("phc_gemm_tc5: C_hi/C_lo come as a pair and not with accumulate"); return PHC_ERR_INVALID_ARG; }
   static Params P;
   memset(&P, 0, sizeof(P));
-  P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, lda, a_kmajor, B_hi, B_lo, ldb, b_kmajor, C, C_hi, C_lo, ldc, M, N, K, alpha, bias,
+  P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, lda, a_kmajor, B_hi, B_lo, nullptr, ldb, b_kmajor, C, C_hi, C_lo, ldc, M, N, K, alpha, bias,
                               relu, mask, ldmask, accumulate, k_splits);
   P.count = 1;
   return launch<128, true>(P, false, false, static_cast<cudaStream_t>(stream));
@@ -650,6 +834,38 @@ extern "C" int phc_split_tf32(const float* x, int64_t ldx, int64_t rows, int32_t
   phc::wg::split_tf32_kernel<<<(unsigned)g, 256, 0, static_cast<cudaStream_t>(stream)>>>(x, ldx, rows, cols, hi, lo, ldo);
   phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "split_tf32_kernel");
+}
+
+extern "C" int64_t phc_gemm_image_floats(int32_t N, int32_t K) {
+  return N < 1 || K < 1 ? 0 : phc::wg::image_blocks(N, K) * phc::wg::IMG_BLOCK;
+}
+
+extern "C" int phc_gemm_make_images(const PhcGemmImageDesc* d, int32_t count, void* stream) {
+  using namespace phc::wg;
+  if (count < 0 || (count > 0 && !d)) { phc_set_error("phc_gemm_make_images: bad arguments"); return PHC_ERR_INVALID_ARG; }
+  for (int i = 0; i < count; ++i) {
+    const PhcGemmImageDesc& g = d[i];
+    if (!g.B || !g.img || g.N < 1 || g.K < 1 || g.ldb < (g.b_kmajor ? g.K : g.N)) { phc_set_error("phc_gemm_make_images: bad image (NULL pointer, empty or ldb too small)"); return PHC_ERR_INVALID_ARG; }
+    if (reinterpret_cast<uintptr_t>(g.img) & 15) { phc_set_error("phc_gemm_make_images: img must be 16-byte aligned"); return PHC_ERR_INVALID_ARG; }
+  }
+  static ImgParams P;
+  for (int i0 = 0; i0 < count; i0 += IMG_JOBS) {
+    memset(&P, 0, sizeof(P));
+    P.count = count - i0 < IMG_JOBS ? count - i0 : IMG_JOBS;
+    long long blocks = 0;
+    for (int i = 0; i < P.count; ++i) {
+      const PhcGemmImageDesc& g = d[i0 + i];
+      P.j[i] = ImgJob{g.B, (long long)g.ldb, g.img, blocks, g.b_kmajor ? 1 : 0, g.N, g.K, (g.K + IMG_BK - 1) / IMG_BK};
+      blocks += image_blocks(g.N, g.K);
+    }
+    P.total_blocks = blocks;
+    const long long grid = blocks < 132 * 8 ? blocks : 132 * 8;
+    weight_image_kernel<<<(unsigned)grid, NUM_THREADS, 0, static_cast<cudaStream_t>(stream)>>>(P);
+    phc_count_launches(1);
+    const int rc = phc_check_cuda(cudaGetLastError(), "weight_image_kernel launch");
+    if (rc != PHC_OK) return rc;
+  }
+  return PHC_OK;
 }
 
 extern "C" int phc_split_lo(const float* x, float* lo, int64_t n, void* stream) {

@@ -267,7 +267,7 @@ class AMPAgent:
                                 ending_act=bool(netcfg.get("ending_act", True)))
         if self.multi_gpu:
             D.broadcast_params(self.model.params, 0)
-            self.model._lo_version = -1                 # the collective wrote the bucket behind torch's version counter
+            self.model.refresh_images()                 # the collective wrote the bucket behind torch's version counter
         # mlp_precision: "fp32" (3xTF32, the reference's mixed_precision: False) or "tf32" (single tensor-core pass, opt-in)
         self.engine = MLPEngine(self.model, precision=str(cfg.get("mlp_precision", "fp32")))
         n = self.model.num_floats
@@ -698,6 +698,8 @@ class AMPAgent:
                                          net.num_floats, self._gsumsq.data_ptr(), grad_scale,
                                          self.grad_norm if self.truncate_grads else 0.0, self.last_lr, 0.9, 0.999, 1e-8,
                                          self.opt_step, st))
+            if self.engine.uses_images:
+                net.refresh_images()
             if self.engine.backend == "tc5":
                 net.refresh_split()                    # hi/lo operand copies of the updated weights
 
@@ -854,13 +856,14 @@ class AMPAgent:
         steps = []
         for li in range(L - 1, 0, -1):
             l = hid[li]
-            steps.append(([eng.gdesc(u[li], True, net.weight(l), False, u[li - 1], Bd, l.in_dim, l.out_dim, **mask(li - 1))], None))
+            steps.append(([eng.gdesc(u[li], True, net.weight(l), False, u[li - 1], Bd, l.in_dim, l.out_dim, B_img=eng.image(l, False),
+                                     **mask(li - 1))], None))
         l0 = hid[0]
         c = self._disc_coef * self._disc_grad_penalty
 
         def penalty():
             _lib.check(lib.phc_scale_sumsq(g.data_ptr(), g.stride(0), Bd, l0.in_dim, 2.0 * c / Bd, self._stats[10:].data_ptr(), st))
-        steps.append(([eng.gdesc(u[0], True, net.weight(l0), False, g, Bd, l0.in_dim, l0.out_dim)], penalty))
+        steps.append(([eng.gdesc(u[0], True, net.weight(l0), False, g, Bd, l0.in_dim, l0.out_dim, B_img=eng.image(l0, False))], penalty))
         for li in range(L):
             l = hid[li]
             src = g if li == 0 else e[li - 1]
@@ -868,7 +871,8 @@ class AMPAgent:
             if li == L - 1:
                 after = lambda: eng.colsum(e[L - 1], Bd, hid[L - 1].out_dim, net.weight(head, True))
             steps.append(([eng.gdesc(u[li], False, src, False, net.weight(l, True), l.out_dim, l.in_dim, Bd, accumulate=True, k_splits=group_splits(Bd)),
-                           eng.gdesc(src, True, net.weight(l), True, e[li], Bd, l.out_dim, l.in_dim, **mask(li))], after))
+                           eng.gdesc(src, True, net.weight(l), True, e[li], Bd, l.out_dim, l.in_dim, B_img=eng.image(l, True), **mask(li))],
+                          after))
         return steps
 
     def _disc_grad_penalty_backward(self, x_demo: torch.Tensor, h_demo, Bd: int) -> None:

@@ -60,6 +60,7 @@ def load_pnn(checkpoint: Dict, num_prim: int, has_lateral: bool = False, activat
     for col in net.pnn_actors:
         for l in col.layers:
             net.set_layer(l, sd[f"a2c_network.{l.name}.weight"], sd[f"a2c_network.{l.name}.bias"])
+    net.refresh_images()
     eng = MLPEngine(net, backend)
     if eng.backend == "tc5":
         net.refresh_split()

@@ -35,6 +35,8 @@ class LinearSpec:
     out_dim: int
     w_off: int = 0     # offsets into the flat bucket (floats)
     b_off: int = 0
+    img_fwd: int = 0   # offsets of the layer's weight images in AMPNetwork.images (floats)
+    img_dx: int = 0
 
     @property
     def in_pad(self) -> int:
@@ -113,12 +115,43 @@ class AMPNetwork:
         self.params_hi = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.params_lo = torch.zeros(off, dtype=torch.float32, device=self.device)
         self.sigma = torch.full((action_dim,), float(sigma_init), dtype=torch.float32, device=self.device)
+        # weight images (include/phc_b200.h, PhcGemmDesc.B_img) of every layer in both of the GEMM's weight-side forms: the
+        # forward (B = W: N = out, K = in) and dX (B = W read MN-major: N = in, K = out)
+        lib, off, descs = _lib.load(), 0, []
+        for l in self.all_layers():
+            l.img_fwd = off
+            off += lib.phc_gemm_image_floats(l.out_dim, l.in_dim)
+            l.img_dx = off
+            off += lib.phc_gemm_image_floats(l.in_dim, l.out_dim)
+        self.images = torch.zeros(off, dtype=torch.float32, device=self.device)
+        for l in self.all_layers():
+            W = self.weight(l)
+            descs += [_lib.PhcGemmImageDesc(W.data_ptr(), W.stride(0), 1, l.out_dim, l.in_dim, self.images[l.img_fwd:].data_ptr()),
+                      _lib.PhcGemmImageDesc(W.data_ptr(), W.stride(0), 0, l.in_dim, l.out_dim, self.images[l.img_dx:].data_ptr())]
+        self._image_descs = (_lib.PhcGemmImageDesc * len(descs))(*descs)
+        self._images_of = None            # params._version the images were made from
         self._init_default(seed)
+        self.refresh_images()
 
     # ---- views -------------------------------------------------------------------------------------------
     def weight(self, l: LinearSpec, grad: bool = False, part: Optional[str] = None) -> torch.Tensor:
         buf = self.grads if grad else {None: self.params, "hi": self.params_hi, "lo": self.params_lo}[part]
         return buf[l.w_off:l.w_off + l.out_dim * l.in_pad].view(l.out_dim, l.in_pad)
+
+    def image(self, l: LinearSpec, kmajor: bool) -> torch.Tensor:
+        """The weight image of layer l as the forward's B (kmajor) or dX's B; remade first if params was written through torch
+        since the last refresh_images()."""
+        if self._images_of != self.params._version:
+            self.refresh_images()
+        return self.images[l.img_fwd if kmajor else l.img_dx:]
+
+    def refresh_images(self) -> None:
+        """Remake every weight image from params, in one launch.  A stale image gives silently wrong products, so every writer
+        of params calls this: construction, load_state_dict, the optimiser step (where the engine reads images) and the
+        multi-GPU broadcast.  Writes through
+        torch are also caught by image(), from the bucket's version counter; writes through raw pointers are not."""
+        _lib.check(_lib.load().phc_gemm_make_images(self._image_descs, len(self._image_descs), _stream()), "phc_gemm_make_images")
+        self._images_of = self.params._version
 
     def refresh_split(self) -> None:
         """hi = rna_tf32(W), lo = rna_tf32(W - hi) over the whole bucket (one streaming pass, 5.5 M floats)."""
@@ -173,6 +206,7 @@ class AMPNetwork:
             self.set_layer(l, sd[f"{prefix}{l.name}.weight"], sd[f"{prefix}{l.name}.bias"])
         if prefix + "sigma" in sd:
             self.sigma.copy_(sd[prefix + "sigma"].to(self.device))
+        self.refresh_images()
 
     def get_disc_logit_weights(self) -> torch.Tensor:
         return self.weight(self.disc.head)[:, :self.disc.head.in_dim].flatten()
@@ -218,6 +252,8 @@ class MLPEngine:
             raise ValueError("precision='tf32' (single tensor-core pass) exists on the tc5s back end only")
         self._companions: Dict[Tuple[int, Tuple[int, ...], Tuple[int, ...]], Tuple[torch.Tensor, torch.Tensor]] = {}
         self.gemm_flops = 0.0          # algorithmic fp32 FLOPs (2 M N K) of every grouped launch so far (bench.py reads it)
+        # the weight images feed the grouped 3xTF32 launches; the single-pass kernel stages B itself and never reads them
+        self.uses_images = self.backend == "tc5s" and precision == "fp32"
         if self.backend == "tc5":
             net.refresh_split()
 
@@ -282,10 +318,15 @@ class MLPEngine:
             _lib.check(rc, "phc_gemm")
 
     # -- grouped launches (tc5s only): one persistent kernel over the tiles of up to PHC_GEMM_GROUP_MAX independent GEMMs ------
-    def gdesc(self, A, a_k, B, b_k, C, M, N, K, alpha=1.0, bias=None, act=0, aux=None, accumulate=False, k_splits=1):
+    def image(self, l: LinearSpec, kmajor: bool) -> Optional[torch.Tensor]:
+        """layer l's weight image for the forward (kmajor) or dX form, or None where the launches do not read images"""
+        return self.net.image(l, kmajor) if self.uses_images else None
+
+    def gdesc(self, A, a_k, B, b_k, C, M, N, K, alpha=1.0, bias=None, act=0, aux=None, accumulate=False, k_splits=1, B_img=None):
+        """B_img: B's weight image for this N and K (AMPNetwork.image), or None to stage B from the fp32 operand."""
         return _lib.PhcGemmDesc(A.data_ptr(), A.stride(0), 1 if a_k else 0, B.data_ptr(), B.stride(0), 1 if b_k else 0, C.data_ptr(),
                                 C.stride(0), M, N, K, alpha, _ptr(bias), act, _ptr(aux), aux.stride(0) if aux is not None else 0,
-                                1 if accumulate else 0, k_splits, None)
+                                1 if accumulate else 0, k_splits, None, _ptr(B_img))
 
     def fwd_desc(self, st: MLPStack, li: int, x: torch.Tensor, ws: Dict[str, torch.Tensor]):
         """Layer li of the forward pass of stack st on batch x / workspace ws (the same epilogues as forward())."""
@@ -300,7 +341,8 @@ class MLPEngine:
             out = ws["out"]
             act = _lib.PHC_ACT_NONE if not st.head_relu else (_lib.PHC_ACT_SILU if silu else (_lib.PHC_ACT_RELU_BITS if "obits" in ws else _lib.PHC_ACT_RELU))
             aux = None if not st.head_relu else (ws["z_out"] if silu else ws.get("obits"))
-        return self.gdesc(inp, True, net.weight(l), True, out, B, l.out_dim, l.in_dim, bias=net.bias(l), act=act, aux=aux)
+        return self.gdesc(inp, True, net.weight(l), True, out, B, l.out_dim, l.in_dim, bias=net.bias(l), act=act, aux=aux,
+                          B_img=self.image(l, True))
 
     def bwd_descs(self, st: MLPStack, li: int, x: torch.Tensor, ws: Dict[str, torch.Tensor], dx: Optional[torch.Tensor] = None):
         """(dW, dX) problems of layer li: dW[out, in] += dY^T X (split-K, reduce-add into the gradient bucket) and
@@ -310,15 +352,16 @@ class MLPEngine:
         inp = x if li == 0 else ws["h"][li - 1]
         dw = self.gdesc(dY, False, inp, False, net.weight(l, grad=True), l.out_dim, l.in_dim, B, accumulate=True, k_splits=group_splits(B))
         dxd = None
+        img = self.image(l, False)
         if li > 0:
             if st.activation == "silu":
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_SILU_BWD, aux=ws["z"][li - 1])
+                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_SILU_BWD, aux=ws["z"][li - 1], B_img=img)
             elif "hbits" in ws:
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_MASK_BITS, aux=ws["hbits"][li - 1])
+                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_MASK_BITS, aux=ws["hbits"][li - 1], B_img=img)
             else:
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, aux=ws["h"][li - 1])
+                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, aux=ws["h"][li - 1], B_img=img)
         elif dx is not None:
-            dxd = self.gdesc(dY, True, net.weight(l), False, dx, B, l.in_dim, l.out_dim)
+            dxd = self.gdesc(dY, True, net.weight(l), False, dx, B, l.in_dim, l.out_dim, B_img=img)
         return dw, dxd
 
     def _set_mode(self) -> None:
@@ -379,6 +422,9 @@ class MLPEngine:
 
     # -- forward: x is [B, in_pad] (zero padded) -------------------------------------------------------------------
     def forward(self, st: MLPStack, x: torch.Tensor, ws: Dict[str, torch.Tensor]) -> torch.Tensor:
+        if self.backend == "tc5s":                          # the grouped launch, so that B comes from the weight images
+            self.forward_group([(st, x, ws)])
+            return ws["out"]
         net, B = self.net, x.shape[0]
         tc5 = self.backend == "tc5"
         cur, cur_split = x, (self.split(x) if tc5 else None)

@@ -35,12 +35,25 @@ import bench  # noqa: E402
 from phc_b200 import _lib  # noqa: E402
 
 
+class GemmDescNoImage(C.Structure):
+    """PhcGemmDesc of a build from before the weight images (no B_img field)."""
+    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] != "B_img"]
+
+
 def open_lib(path):
     lib = C.CDLL(os.path.abspath(path))
     for name in ("phc_gemm_group", "phc_gemm_set_precision", "phc_gemm_tc5s_set_tile", "phc_gemm_tc5s_set_sched", "phc_last_error"):
         res, args = _lib.SIGNATURES[name]
         getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
+    # each build gets descriptors in its own layout; one without images computes the same problems from the staged operands
+    lib.desc_type = _lib.PhcGemmDesc if hasattr(lib, "phc_gemm_make_images") else GemmDescNoImage
+    lib.phc_gemm_group.argtypes = [C.POINTER(lib.desc_type), C.c_int32, C.c_void_p]
     return lib
+
+
+def desc_array(lib, descs):
+    T = lib.desc_type
+    return (T * len(descs))(*[T(*[getattr(d, f) for f, _ in T._fields_]) for d in descs])
 
 
 def gpu_info():
@@ -99,12 +112,12 @@ def main():
     fwd_roll = [[eng.fwd_desc(st, li, xin, ws) for st, xin, ws in roll if li < len(st.layers)] for li in range(depth)]
     groups = [(f"fwd L{li}", g) for li, g in enumerate(fwd)] + [(f"bwd L-{k + 1}", g) for k, g in enumerate(bwd)]
     groups += [(f"rollout fwd L{li} ({n_roll} rows)", g) for li, g in enumerate(fwd_roll)]
-    arrays = {name: ((_lib.PhcGemmDesc * len(g))(*g), len(g)) for name, g in groups}
+    arrays = {key: {name: (desc_array(lib, g), len(g)) for name, g in groups} for key, lib in libs.items()}
     for name, g in groups:
         assert len(g) <= _lib.PHC_GEMM_GROUP_MAX, name
 
     def launch(lib, name):
-        arr, n = arrays[name]
+        arr, n = arrays["A" if lib is libs["A"] else "B"][name]
         rc = lib.phc_gemm_group(arr, n, C.c_void_p(torch.cuda.current_stream().cuda_stream))
         if rc:
             raise RuntimeError(f"phc_gemm_group({name}) = {rc}: {lib.phc_last_error().decode()}")
