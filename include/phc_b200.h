@@ -453,10 +453,15 @@ typedef struct PhcGemmDesc {
   const float* B_lo;        /* optional: the 3xTF32 low part of B, same layout and ldb, made by phc_split_lo; validated and not
                              * read (the kernel makes the identical low part from the tiles it stages) */
   const float* B_img;       /* optional: B's weight image for this problem's N and K (phc_gemm_make_images), 16-byte aligned, with
-                             * a_kmajor only.  With 128 x 128 tiles the kernel then reads B from the image (one bulk copy per
+                             * a_kmajor or A_img.  With 128 x 128 tiles the kernel then reads B from the image (one bulk copy per
                              * k-block) and A straight into the tensor-core registers instead of staging both; the result is the
                              * same bit for bit.  128 x 256 tiles and PHC_GEMM_TF32_SINGLE_PASS ignore it.  The image must be
                              * remade whenever B changes. */
+  const float* A_img;       /* optional, only with B_img: A's image in the same layout with rows = M (phc_gemm_make_images with
+                             * B = A, N = M, b_kmajor = a_kmajor), 16-byte aligned.  With both images the kernel reads both operands
+                             * by bulk copy and never looks at a_kmajor / b_kmajor; the result is again the same bit for bit, and
+                             * the same two cases ignore both images.  Meant for the weight gradient (dW += dY^T X, both operands
+                             * mn-major activations), whose images are made once per launch instead of staged once per tile. */
 } PhcGemmDesc;
 /* Weight image of a B operand (B(n,k) as in PhcGemmDesc, N x K): one block of 8192 floats per (128-row n-tile nt, 32-wide k-block
  * kb), block nt * ceil(K / 32) + kb, each block [hi | lo] of 4096 floats with hi = trunc_tf32(B), lo = rna_tf32(B - hi) (the

@@ -25,7 +25,9 @@
 // draws its tiles dynamically; a slice then only waits for a lower-numbered tile that a running CTA has already drawn.
 // phc_gemm_tc5 is the same kernel with operands pre-split in global memory (hi / lo arrays loaded instead of split).
 // A 3xTF32 problem with 128 x 128 tiles that comes with a weight image of B (PhcGemmDesc.B_img) skips the staging: B arrives
-// pre-split by bulk copy and A goes from global memory straight into the wgmma register fragment (the image loop below).
+// pre-split by bulk copy and A goes from global memory straight into the wgmma register fragment (the image loop below).  One
+// that also comes with an image of A (PhcGemmDesc.A_img: the weight gradient, whose operands are both mn-major activations,
+// imaged once per launch instead of once per tile) takes both operands by bulk copy into the staged loop's stages (the pair loop).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -68,6 +70,7 @@ constexpr int IMG_STAGES = 4;             // B ring of the image loop: 4 x 32 KB
 struct Prob {
   const float* A; const float* B; const float* A_lo; const float* B_lo;      // A_lo / B_lo: pre-split operands (phc_gemm_tc5)
   const float* B_img;                                                          // weight image of B (128 x 128 tiles only), or NULL
+  const float* A_img;                                                          // image of A (only with B_img), or NULL
   float* C; float* C_hi; float* C_lo;                                          // C_hi / C_lo: split copies of the result (phc_gemm_tc5)
   const float* bias;
   float* aux;
@@ -275,18 +278,24 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
   constexpr int MODE = SINGLE ? 1 : PRESPLIT ? 2 : 0;
   // single pass stays on the staged loop: ptxas serialises the wgmmas of its image loop (C7513)
   constexpr bool HAS_IMG = BN == IMG_ROWS && BK == IMG_BK && !PRESPLIT && !SINGLE;
+  static_assert(!HAS_IMG || (C::A_TILE == IMG_HALF * 4 && C::B_TILE == IMG_HALF * 4), "an image block pair is one stage");
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ int s_tile;
   __shared__ __align__(8) uint64_t s_bar[IMG_STAGES];      // one mbarrier per B stage of the image loop
+  __shared__ __align__(8) uint64_t s_pbar[C::STAGES];      // one mbarrier per stage of the pair loop
   const int tid = threadIdx.x, lane = tid & 31, wgi = tid >> 7, wq = (tid >> 5) & 3;
   const uint32_t sbase = (uint32_t)__cvta_generic_to_shared(smem);
   const uint32_t bar0 = (uint32_t)__cvta_generic_to_shared(s_bar);
+  const uint32_t pbar0 = (uint32_t)__cvta_generic_to_shared(s_pbar);
   const bool dyn = P.sched != nullptr;
   int ring = 0;                                             // k-blocks the image loop has taken through its B ring so far
+  uint32_t pphase = 0;                                      // bit s: the parity the pair loop waits for next on stage s
   if constexpr (HAS_IMG) {
     if (tid == 0) {
 #pragma unroll
       for (int s = 0; s < IMG_STAGES; ++s) mbar_init(bar0 + 8 * s, 1);
+#pragma unroll
+      for (int s = 0; s < C::STAGES; ++s) mbar_init(pbar0 + 8 * s, 1);
       mbar_init_fence();
     }
     __syncthreads();
@@ -318,9 +327,57 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
     float acc[BN / 2];
 #pragma unroll
     for (int j = 0; j < BN / 2; ++j) acc[j] = 0.f;
+    // k-block j of the staged and the pair loop sits in shared-memory stage j % 3 as [A hi | A lo | B hi | B lo]
+    auto stage = [&](int j) { return sbase + (uint32_t)((j % C::STAGES) * C::STAGE); };
+    auto mma = [&](int j) {                                  // one wgmma batch: every product of k-block j
+      const uint32_t s = stage(j);
+      const uint32_t a_hi = s + (uint32_t)(wgi * 8 * C::SBO), a_lo = a_hi + C::A_TILE;
+      const uint32_t b_hi = s + 2 * C::A_TILE, b_lo = b_hi + C::B_TILE;
+      wgmma_fence();
+#pragma unroll
+      for (int kk = 0; kk < BK / 8; ++kk) {
+        const uint32_t o = (uint32_t)kk * 256u;
+        const uint64_t dAh = smem_desc(a_hi + o, 128, C::SBO), dBh = smem_desc(b_hi + o, 128, C::SBO);
+        if constexpr (!SINGLE) {
+          wgmma_tf32<BN>(acc, smem_desc(a_lo + o, 128, C::SBO), dBh);
+          wgmma_tf32<BN>(acc, dAh, smem_desc(b_lo + o, 128, C::SBO));
+        }
+        wgmma_tf32<BN>(acc, dAh, dBh);
+      }
+      wgmma_commit();
+    };
     bool staged = true;
     if constexpr (HAS_IMG) {
-      if (q.B_img != nullptr) {                              // (uniform) B from its weight image, A from registers
+      if (q.A_img != nullptr) {                              // (uniform) A and B both from their images: the pair loop
+        staged = false;
+        // The A block and the B block of a k-block are [hi | lo] 32 KB each, in the layout the staged loop writes, so together
+        // they fill one stage exactly and the staged loop's mma(j) consumes it: the products, their order and the k order are
+        // the staged loop's, and the results are the same bit for bit.  Thread 0 fills stage j % 3 with two bulk copies under
+        // that stage's mbarrier, 3 k-blocks ahead; the barrier after wait_group 1 of step j frees the stage of j - 1.  No
+        // generic-proxy write touches the stages, so there is no proxy fence.  The stages' mbarriers are not the image loop's:
+        // their phases are counted per stage in pphase, whatever ring position the image loop is at.
+        const float* aimg = q.A_img + (long long)mi * q.kb_total * IMG_BLOCK;
+        const float* bimg = q.B_img + (long long)ni * q.kb_total * IMG_BLOCK;
+        auto issue = [&](int j) {
+          const uint32_t s = stage(j), bar = pbar0 + 8 * (j % C::STAGES);
+          mbar_expect_tx(bar, C::STAGE);
+          bulk_g2s(s, aimg + (long long)(kb_begin + j) * IMG_BLOCK, IMG_BLOCK * 4, bar);
+          bulk_g2s(s + 2 * C::A_TILE, bimg + (long long)(kb_begin + j) * IMG_BLOCK, IMG_BLOCK * 4, bar);
+        };
+        if (tid == 0)
+          for (int j = 0; j < min(nkb, C::STAGES); ++j) issue(j);
+#pragma unroll 1
+        for (int j = 0; j < nkb; ++j) {
+          const int s = j % C::STAGES;
+          mbar_wait(pbar0 + 8 * s, (pphase >> s) & 1u);
+          pphase ^= 1u << s;
+          mma(j);
+          wgmma_wait<1>();
+          __syncthreads();
+          if (tid == 0 && j >= 1 && j + 2 < nkb) issue(j + 2);
+        }
+        wgmma_wait<0>();
+      } else if (q.B_img != nullptr) {                       // (uniform) B from its weight image, A from registers
         staged = false;
         // B: k-block j arrives in ring slot (ring + j) % IMG_STAGES by one bulk copy that thread 0 issues, IMG_STAGES k-blocks
         // ahead; the barrier after wait_group 1 of step j says that the slot of j - 1 is free again.  No generic-proxy write
@@ -414,7 +471,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
           load_op<BN, BK>(v.b_lo, q.B_lo, q.ldb, bk, n0, q.N, k0, q.K, tid);
         }
       };
-      auto stage = [&](int j) { return sbase + (uint32_t)((j % C::STAGES) * C::STAGE); };
       auto store = [&](int j) {
         const uint32_t s = stage(j);
         if constexpr (PRESPLIT) {
@@ -425,23 +481,6 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
           store_op<BN, BK, C::B_PER, MODE>(v.b, v.b, s + 2 * C::A_TILE, s + 2 * C::A_TILE + C::B_TILE, bk, tid);
         }
         fence_async_smem();                                   // generic-proxy writes -> visible to the tensor core's reads
-      };
-      auto mma = [&](int j) {                                  // one wgmma batch: every product of k-block j
-        const uint32_t s = stage(j);
-        const uint32_t a_hi = s + (uint32_t)(wgi * 8 * C::SBO), a_lo = a_hi + C::A_TILE;
-        const uint32_t b_hi = s + 2 * C::A_TILE, b_lo = b_hi + C::B_TILE;
-        wgmma_fence();
-  #pragma unroll
-        for (int kk = 0; kk < BK / 8; ++kk) {
-          const uint32_t o = (uint32_t)kk * 256u;
-          const uint64_t dAh = smem_desc(a_hi + o, 128, C::SBO), dBh = smem_desc(b_hi + o, 128, C::SBO);
-          if constexpr (!SINGLE) {
-            wgmma_tf32<BN>(acc, smem_desc(a_lo + o, 128, C::SBO), dBh);
-            wgmma_tf32<BN>(acc, dAh, smem_desc(b_lo + o, 128, C::SBO));
-          }
-          wgmma_tf32<BN>(acc, dAh, dBh);
-        }
-        wgmma_commit();
       };
       // Step j: k-block j's wgmmas go out; k-block j + 1, loaded during step j - 1, is split and stored into the stage of
       // j - 2, whose wgmmas the barrier of step j - 1 saw finish; then the loads of j + 2 are issued.  They come after the store
@@ -491,6 +530,17 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
         if (nb >= q.N) break;                                // warp-uniform
         const uint32_t mbits = (act == PHC_ACT_MASK_BITS && brow) ? brow[nb >> 5] : 0u;
         uint32_t bits = 0;
+        // ordered: this tile is C's only writer right now.  The chunk's old C values are read past L1 all at once, before any
+        // store, so that their L2 round trips overlap: the turnstile chains the epilogues of an output tile's slices one after
+        // the other, so the latency of each epilogue adds up over the slices.
+        float old[8];
+        if (ordered && row_ok) {
+#pragma unroll
+          for (int e = 0; e < 8; ++e) {
+            const int n = nb + 8 * (e >> 1) + 2 * (lane & 3) + (e & 1);
+            old[e] = n < q.N ? __ldcg(crow + n) : 0.f;
+          }
+        }
 #pragma unroll
         for (int jj = 0; jj < 4; ++jj) {
           const int j = 4 * qc + jj;
@@ -515,9 +565,9 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
           }
           if (!row_ok) continue;
           const int n = nb + nl;
-          if (ordered) {                                     // this tile's only writer right now: read C past L1, add, store
-            if (n < q.N) crow[n] = __ldcg(crow + n) + v[0];
-            if (n + 1 < q.N) crow[n + 1] = __ldcg(crow + n + 1) + v[1];
+          if (ordered) {
+            if (n < q.N) crow[n] = old[2 * jj] + v[0];
+            if (n + 1 < q.N) crow[n + 1] = old[2 * jj + 1] + v[1];
           } else if (q.accumulate) {                         // one writer per element: same result whatever the order
             if (n < q.N) atomicAdd(crow + n, v[0]);
             if (n + 1 < q.N) atomicAdd(crow + n + 1, v[1]);
@@ -618,12 +668,13 @@ static int num_sms() {
 }
 
 // fills P.p[n] for one problem; returns the number of tiles it adds
-static int add_problem(Params& P, int n, int tiles, int bn, const float* A, const float* A_lo, long long lda, int a_k, const float* B,
-                       const float* B_lo, const float* B_img, long long ldb, int b_k, float* Cm, float* C_hi, float* C_lo, long long ldc, int M, int N, int K,
+static int add_problem(Params& P, int n, int tiles, int bn, const float* A, const float* A_lo, const float* A_img, long long lda, int a_k,
+                       const float* B, const float* B_lo, const float* B_img, long long ldb, int b_k, float* Cm, float* C_hi, float* C_lo, long long ldc, int M, int N, int K,
                        float alpha, const float* bias, int act, float* aux, long long ldaux, int accumulate, int k_splits) {
   const int bk = bn == 128 ? Cfg<128>::BK : Cfg<256>::BK;
   Prob& q = P.p[n];
-  q.A = A; q.A_lo = A_lo; q.B = B; q.B_lo = B_lo; q.B_img = bn == IMG_ROWS ? B_img : nullptr; q.C = Cm; q.C_hi = C_hi; q.C_lo = C_lo; q.bias = bias; q.aux = aux;
+  q.A = A; q.A_lo = A_lo; q.B = B; q.B_lo = B_lo; q.B_img = bn == IMG_ROWS ? B_img : nullptr;
+  q.A_img = q.B_img ? A_img : nullptr; q.C = Cm; q.C_hi = C_hi; q.C_lo = C_lo; q.bias = bias; q.aux = aux;
   q.lda = lda; q.ldb = ldb; q.ldc = ldc; q.ldaux = ldaux; q.M = M; q.N = N; q.K = K; q.alpha = alpha; q.act = act;
   q.accumulate = accumulate ? 1 : 0; q.a_k = a_k ? 1 : 0; q.b_k = b_k ? 1 : 0;
   int ks = k_splits < 1 ? 1 : k_splits;
@@ -740,7 +791,8 @@ static int validate_group(const PhcGemmDesc* d, int32_t count) {
     if (g.act >= PHC_ACT_RELU_BITS && g.aux && ((reinterpret_cast<uintptr_t>(g.aux) & 3) || g.ldaux < (g.N + 31) / 32)) { phc_set_error("phc_gemm_group: bit-mask aux needs ldaux >= ceil(N / 32) words"); return PHC_ERR_INVALID_ARG; }
     if (ks > 1 && (!g.accumulate || g.act || g.aux)) { phc_set_error("phc_gemm_group: split-K needs accumulate=1 and a linear epilogue"); return PHC_ERR_INVALID_ARG; }
     if (g.B_lo && (reinterpret_cast<uintptr_t>(g.B_lo) & 15)) { phc_set_error("phc_gemm_group: B_lo must be 16-byte aligned"); return PHC_ERR_INVALID_ARG; }
-    if (g.B_img && ((reinterpret_cast<uintptr_t>(g.B_img) & 15) || !g.a_kmajor)) { phc_set_error("phc_gemm_group: B_img must be 16-byte aligned and comes with a_kmajor only"); return PHC_ERR_INVALID_ARG; }
+    if (g.A_img && ((reinterpret_cast<uintptr_t>(g.A_img) & 15) || !g.B_img)) { phc_set_error("phc_gemm_group: A_img must be 16-byte aligned and comes with B_img only"); return PHC_ERR_INVALID_ARG; }
+    if (g.B_img && ((reinterpret_cast<uintptr_t>(g.B_img) & 15) || (!g.a_kmajor && !g.A_img))) { phc_set_error("phc_gemm_group: B_img must be 16-byte aligned and comes with a_kmajor or A_img only"); return PHC_ERR_INVALID_ARG; }
   }
   // write hazards: the C spans [C, C + (M - 1) ldc + N) of two problems may only overlap when both accumulate into the same C with
   // the same shape -- they then share a turnstile and add in problem order; any other overlap would race (plain stores, or
@@ -782,7 +834,7 @@ extern "C" int phc_gemm_group(const PhcGemmDesc* d, int32_t count, void* stream)
   for (int i = 0; i < count; ++i) {
     const PhcGemmDesc& g = d[i];
     if (g.M == 0 || g.N == 0) continue;
-    tiles += add_problem(P, n, tiles, bn, g.A, nullptr, g.lda, g.a_kmajor, g.B, nullptr, g.B_img, g.ldb, g.b_kmajor, g.C, nullptr, nullptr, g.ldc,
+    tiles += add_problem(P, n, tiles, bn, g.A, nullptr, g.A_img, g.lda, g.a_kmajor, g.B, nullptr, g.B_img, g.ldb, g.b_kmajor, g.C, nullptr, nullptr, g.ldc,
                          g.M, g.N, g.K, g.alpha, g.bias, g.act, g.aux, g.ldaux, g.accumulate, g.k_splits);
     ++n;
   }
@@ -799,7 +851,7 @@ extern "C" int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, cons
   PhcGemmDesc d;
   d.A = A; d.lda = lda; d.a_kmajor = a_kmajor; d.B = B; d.ldb = ldb; d.b_kmajor = b_kmajor; d.C = C; d.ldc = ldc;
   d.M = M; d.N = N; d.K = K; d.alpha = alpha; d.bias = bias; d.act = act; d.aux = aux; d.ldaux = ldaux;
-  d.accumulate = accumulate; d.k_splits = k_splits; d.B_lo = nullptr; d.B_img = nullptr;
+  d.accumulate = accumulate; d.k_splits = k_splits; d.B_lo = nullptr; d.B_img = nullptr; d.A_img = nullptr;
   return phc_gemm_group(&d, 1, stream);
 }
 
@@ -820,7 +872,7 @@ extern "C" int phc_gemm_tc5(const float* A_hi, const float* A_lo, int64_t lda, i
   if ((C_hi == nullptr) != (C_lo == nullptr) || (C_hi && accumulate)) { phc_set_error("phc_gemm_tc5: C_hi/C_lo come as a pair and not with accumulate"); return PHC_ERR_INVALID_ARG; }
   static Params P;
   memset(&P, 0, sizeof(P));
-  P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, lda, a_kmajor, B_hi, B_lo, nullptr, ldb, b_kmajor, C, C_hi, C_lo, ldc, M, N, K, alpha, bias,
+  P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, nullptr, lda, a_kmajor, B_hi, B_lo, nullptr, ldb, b_kmajor, C, C_hi, C_lo, ldc, M, N, K, alpha, bias,
                               relu, mask, ldmask, accumulate, k_splits);
   P.count = 1;
   return launch<128, true>(P, false, false, static_cast<cudaStream_t>(stream));

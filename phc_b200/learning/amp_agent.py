@@ -843,7 +843,6 @@ class AMPAgent:
         _update_grouped merges into its per-layer launches: L input-gradient GEMMs down to g = d logit / d x, the penalty
         itself (phc_scale_sumsq), then per layer the weight-gradient and the forward-form GEMM of the backward chain."""
         lib, net, eng = self._lib, self.model, self.engine
-        from .networks import group_splits
         hid, head = net.disc.hidden, net.disc.head
         L = len(hid)
         ws = self._ws_disc
@@ -870,7 +869,7 @@ class AMPAgent:
             after = None
             if li == L - 1:
                 after = lambda: eng.colsum(e[L - 1], Bd, hid[L - 1].out_dim, net.weight(head, True))
-            steps.append(([eng.gdesc(u[li], False, src, False, net.weight(l, True), l.out_dim, l.in_dim, Bd, accumulate=True, k_splits=group_splits(Bd)),
+            steps.append(([eng.dw_desc(u[li], src, net.weight(l, True), l.out_dim, l.in_dim, Bd),
                            eng.gdesc(src, True, net.weight(l), True, e[li], Bd, l.out_dim, l.in_dim, B_img=eng.image(l, True), **mask(li))],
                           after))
         return steps

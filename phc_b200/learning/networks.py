@@ -254,6 +254,8 @@ class MLPEngine:
         self.gemm_flops = 0.0          # algorithmic fp32 FLOPs (2 M N K) of every grouped launch so far (bench.py reads it)
         # the weight images feed the grouped 3xTF32 launches; the single-pass kernel stages B itself and never reads them
         self.uses_images = self.backend == "tc5s" and precision == "fp32"
+        # activation images of the weight-gradient operands, one buffer per (tensor, rows, K), remade by every launch that reads them
+        self._act_images: Dict[Tuple[int, int, int, int], torch.Tensor] = {}
         if self.backend == "tc5":
             net.refresh_split()
 
@@ -350,7 +352,7 @@ class MLPEngine:
         net, l, B = self.net, st.layers[li], x.shape[0]
         dY = ws["dout"] if li == len(st.layers) - 1 else ws["dh"][li]
         inp = x if li == 0 else ws["h"][li - 1]
-        dw = self.gdesc(dY, False, inp, False, net.weight(l, grad=True), l.out_dim, l.in_dim, B, accumulate=True, k_splits=group_splits(B))
+        dw = self.dw_desc(dY, inp, net.weight(l, grad=True), l.out_dim, l.in_dim, B)
         dxd = None
         img = self.image(l, False)
         if li > 0:
@@ -364,6 +366,40 @@ class MLPEngine:
             dxd = self.gdesc(dY, True, net.weight(l), False, dx, B, l.in_dim, l.out_dim, B_img=img)
         return dw, dxd
 
+    def dw_desc(self, dY: torch.Tensor, X: torch.Tensor, dW: torch.Tensor, M: int, N: int, K: int):
+        """The weight-gradient problem dW[M, N] += dY[:K, :M]^T X[:K, :N], split-K, added into the gradient bucket.  Where the
+        launches read images, it asks for images of dY (A) and X (B): run_group makes them right before the launch."""
+        d = self.gdesc(dY, False, X, False, dW, M, N, K, accumulate=True, k_splits=group_splits(K))
+        # An image costs one pass over its operand (fp32 read, hi / lo written) and saves the split and store of that operand in
+        # every tile across the other dimension.  Timed on the bench minibatch (H100 SXM, 700 W), the layer-0 dW (8 x 8 and 8 x 16
+        # tiles of 128 x 128) is faster with images and the 4 x 8-tile hidden layer and the heads are slower: images are asked for
+        # from tiles_m * tiles_n >= 4 (tiles_m + tiles_n) on.
+        tm, tn = -(-M // 128), -(-N // 128)
+        if self.uses_images and tm * tn >= 4 * (tm + tn):
+            d.image_of = (dY, X)
+        return d
+
+    def make_images(self, descs):
+        """Points A_img / B_img of the descriptors that ask for activation images (dw_desc) at their buffers and returns the
+        image jobs (PhcGemmImageDesc array, count), one per distinct (tensor, rows, K): actor and critic share the input's image."""
+        jobs = {}
+        for d in descs:
+            srcs = getattr(d, "image_of", None)
+            if srcs is None:
+                continue
+            ptrs = []
+            for t, rows in zip(srcs, (d.M, d.N)):
+                key = (t.data_ptr(), t.stride(0), rows, d.K)
+                img = self._act_images.get(key)
+                if img is None:
+                    img = torch.empty(self.lib.phc_gemm_image_floats(rows, d.K), dtype=torch.float32, device=self.dev)
+                    self._act_images[key] = img
+                if key not in jobs:
+                    jobs[key] = _lib.PhcGemmImageDesc(t.data_ptr(), t.stride(0), 0, rows, d.K, img.data_ptr())
+                ptrs.append(img.data_ptr())
+            d.A_img, d.B_img = ptrs
+        return (_lib.PhcGemmImageDesc * len(jobs))(*jobs.values()), len(jobs)
+
     def _set_mode(self) -> None:
         mode = _lib.PHC_GEMM_TF32_SINGLE_PASS if self.precision == "tf32" else _lib.PHC_GEMM_FP32_3XTF32
         if MLPEngine._mode_set != mode:
@@ -375,6 +411,9 @@ class MLPEngine:
         descs = [d for d in descs if d is not None]
         for i in range(0, len(descs), _lib.PHC_GEMM_GROUP_MAX):
             part = descs[i:i + _lib.PHC_GEMM_GROUP_MAX]
+            jobs, n = self.make_images(part)
+            if n:
+                _lib.check(self.lib.phc_gemm_make_images(jobs, n, _stream()), "phc_gemm_make_images")
             self.gemm_flops += sum(2.0 * d.M * d.N * d.K for d in part)
             arr = (_lib.PhcGemmDesc * len(part))(*part)
             rc = self.lib.phc_gemm_group(arr, len(part), _stream())

@@ -13,8 +13,11 @@ commit's build (from the repository root; phc_b200/lib/ is ignored by git, so th
 The launch groups are those of bench.py:gemm_roofline, from an AMPAgent at the bench configuration (4096 envs, im.yaml
 networks): the three forward launches of one 16384-row minibatch (actor, critic, discriminator advance together) and the
 backward launches by layer index (dW split-K into the gradient bucket + dX), then the rollout forward at 4096 rows, then the
-minibatch launches again with 128 x 256 tiles (phc_gemm_tc5s_set_tile(256)).  Each group alternates A and B `--turns` times;
-a turn is `--iters` launches between two CUDA events after a warm-up.  Printed per group: median [min, max] us per launch
+minibatch launches again with 128 x 256 tiles (phc_gemm_tc5s_set_tile(256)).  Each backward launch is also timed split into
+its weight-gradient problems alone ("dW L-k") and its input-gradient problems alone ("dX L-k").  Each group alternates A and B
+`--turns` times; a turn is `--iters` launches between two CUDA events after a warm-up.  A build that takes activation images
+(PhcGemmDesc.A_img) gets them the way MLPEngine.run_group does: one phc_gemm_make_images launch before every launch that reads
+them, inside the timed window.  Printed per group: median [min, max] us per launch
 and the TFLOP/s of tensor work (3 tensor-core products per fp32 product) for A and B, and B / A.
 
 Before any timing, the whole chain (forward, then backward) runs once per build from the same seeded workspaces, and every
@@ -37,23 +40,35 @@ from phc_b200 import _lib  # noqa: E402
 
 class GemmDescNoImage(C.Structure):
     """PhcGemmDesc of a build from before the weight images (no B_img field)."""
-    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] != "B_img"]
+    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] not in ("B_img", "A_img")]
+
+
+class GemmDescNoActImage(C.Structure):
+    """PhcGemmDesc of a build from before the activation images (no A_img field)."""
+    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] != "A_img"]
 
 
 def open_lib(path):
     lib = C.CDLL(os.path.abspath(path))
-    for name in ("phc_gemm_group", "phc_gemm_set_precision", "phc_gemm_tc5s_set_tile", "phc_gemm_tc5s_set_sched", "phc_last_error"):
-        res, args = _lib.SIGNATURES[name]
-        getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
+    for name in ("phc_gemm_group", "phc_gemm_make_images", "phc_gemm_image_floats", "phc_gemm_set_precision", "phc_gemm_tc5s_set_tile", "phc_gemm_tc5s_set_sched", "phc_last_error"):
+        if hasattr(lib, name):
+            res, args = _lib.SIGNATURES[name]
+            getattr(lib, name).restype, getattr(lib, name).argtypes = res, args
     # each build gets descriptors in its own layout; one without images computes the same problems from the staged operands
-    lib.desc_type = _lib.PhcGemmDesc if hasattr(lib, "phc_gemm_make_images") else GemmDescNoImage
+    # (a build that knows A_img names it in its validation message)
+    with open(path, "rb") as f:
+        act_images = b"A_img" in f.read()
+    lib.desc_type = GemmDescNoImage if not hasattr(lib, "phc_gemm_make_images") else _lib.PhcGemmDesc if act_images else GemmDescNoActImage
     lib.phc_gemm_group.argtypes = [C.POINTER(lib.desc_type), C.c_int32, C.c_void_p]
     return lib
 
 
 def desc_array(lib, descs):
     T = lib.desc_type
-    return (T * len(descs))(*[T(*[getattr(d, f) for f, _ in T._fields_]) for d in descs])
+    names = [f for f, _ in T._fields_]
+    # without A_img a build stages the weight gradient from the fp32 operands (it refuses B_img with mn-major A)
+    drop_b = lambda d: "A_img" not in names and bool(d.A_img)  # noqa: E731
+    return (T * len(descs))(*[T(*[None if f == "B_img" and drop_b(d) else getattr(d, f) for f in names]) for d in descs])
 
 
 def gpu_info():
@@ -112,13 +127,23 @@ def main():
     fwd_roll = [[eng.fwd_desc(st, li, xin, ws) for st, xin, ws in roll if li < len(st.layers)] for li in range(depth)]
     groups = [(f"fwd L{li}", g) for li, g in enumerate(fwd)] + [(f"bwd L-{k + 1}", g) for k, g in enumerate(bwd)]
     groups += [(f"rollout fwd L{li} ({n_roll} rows)", g) for li, g in enumerate(fwd_roll)]
-    arrays = {key: {name: (desc_array(lib, g), len(g)) for name, g in groups} for key, lib in libs.items()}
+    is_dw = lambda d: d.accumulate and not d.a_kmajor  # noqa: E731
+    split = [(f"{part} L-{k + 1}", [d for d in g if is_dw(d) == (part == "dW")]) for k, g in enumerate(bwd) for part in ("dW", "dX")]
+    split = [(name, g) for name, g in split if g]                  # the first layer has no dX
+    # activation images: requested by eng.bwd_descs, made by eng.make_images (it also points each dW descriptor at its images)
+    jobs = {name: eng.make_images(g) for name, g in groups + split}
+    arrays = {key: {name: (desc_array(lib, g), len(g)) for name, g in groups + split} for key, lib in libs.items()}
     for name, g in groups:
         assert len(g) <= _lib.PHC_GEMM_GROUP_MAX, name
 
     def launch(lib, name):
         arr, n = arrays["A" if lib is libs["A"] else "B"][name]
-        rc = lib.phc_gemm_group(arr, n, C.c_void_p(torch.cuda.current_stream().cuda_stream))
+        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        if lib.desc_type is _lib.PhcGemmDesc and jobs[name][1]:
+            rc = lib.phc_gemm_make_images(jobs[name][0], jobs[name][1], stream)
+            if rc:
+                raise RuntimeError(f"phc_gemm_make_images({name}) = {rc}: {lib.phc_last_error().decode()}")
+        rc = lib.phc_gemm_group(arr, n, stream)
         if rc:
             raise RuntimeError(f"phc_gemm_group({name}) = {rc}: {lib.phc_last_error().decode()}")
 
@@ -163,7 +188,7 @@ def main():
         set_tile(w)
         print(f"\n128 x {w} tiles: us per launch, median [min, max] of {args.turns} alternating turns of {args.iters} launches")
         print(f"{'group':28s} {'TFLOP':>7s} | {'A us':>24s} {'A TF/s':>7s} | {'B us':>24s} {'B TF/s':>7s} | B/A")
-        for name, g in groups:
+        for name, g in groups + split:
             if w == 256 and name.startswith("rollout"):
                 continue
             flop = 3.0 * sum(2.0 * d.M * d.N * d.K for d in g)
@@ -176,10 +201,30 @@ def main():
                 tot[(w, k, name.split()[0])] = tot.get((w, k, name.split()[0]), 0.0) + med[k]
             cell = lambda k: f"{med[k]:8.1f} [{min(ts[k]):6.1f}, {max(ts[k]):6.1f}] {flop / med[k] / 1e6:7.1f}"  # noqa: E731
             print(f"{name:28s} {flop / 1e12:7.3f} | {cell('A')} | {cell('B')} | {med['B'] / med['A']:.3f}")
-        for part in ("fwd", "bwd", "rollout"):
+        for part in ("fwd", "bwd", "dW", "dX", "rollout"):
             if (w, "A", part) in tot:
                 a, b = tot[(w, "A", part)], tot[(w, "B", part)]
                 print(f"sum of medians, {part:8s}: A {a:9.1f} us   B {b:9.1f} us   B/A {b / a:.3f}")
+
+    # ---- the activation images alone (part of B's backward times above): bytes read (the operands) and written (the images)
+    if libs["B"].desc_type is _lib.PhcGemmDesc:
+        print("\nactivation images of the backward launches (B's phc_gemm_make_images alone)")
+        stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
+        for name, _ in groups:
+            arr, n = jobs[name]
+            if not n:
+                continue
+            rd = sum(4.0 * arr[i].N * arr[i].K for i in range(n))
+            wr = sum(4.0 * libs["B"].phc_gemm_image_floats(arr[i].N, arr[i].K) for i in range(n))
+            e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+            libs["B"].phc_gemm_make_images(arr, n, stream)
+            e0.record()
+            for _ in range(args.iters):
+                libs["B"].phc_gemm_make_images(arr, n, stream)
+            e1.record()
+            torch.cuda.synchronize()
+            us = e0.elapsed_time(e1) * 1e3 / args.iters
+            print(f"{name:28s} {n} images: {us:8.1f} us, read {rd / 1e9:.3f} GB + write {wr / 1e9:.3f} GB = {(rd + wr) / us / 1e3:7.1f} GB/s")
     net.grads.zero_()
     print(f"gpu after: {gpu_info()}")
     if not ok_all:
