@@ -342,6 +342,29 @@ PHC_API int phc_getup_reset(const int64_t* mask, const int64_t* terminate_in, co
 PHC_API int phc_amp_ring_fill(float* ring, int64_t ring_stride, int64_t n, int32_t num_steps, int32_t amp_dim, const int32_t* head_dev,
                       const int64_t* mask, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Imitation evaluation metrics: the per-step part of IMAmpAgent._post_step_eval (phc/learning/im_amp.py:244-363) and of smpl_sim's
+ * compute_metrics_lite, which the reference runs on the host over the per-clip slices [:num_steps - 1] of the stacked
+ * body_pos / body_pos_gt.  ONE launch per eval step, no host sync.  For env e, with d_t = body_pos[e] - body_pos_gt[e] ([J, 3]):
+ *   frame t counts when t < num_steps[e] - 1 (the slice); then, with means over the J bodies,
+ *   acc[e, 0] += mean |d_t[j]|                               mpjpe_g
+ *   acc[e, 1] += mean |d_t[j] - d_t[0]|                      mpjpe_l (root-relative)
+ *   acc[e, 2] += mean |a R^T y_j + mu_gt - gt_j|             mpjpe_pa: pred aligned onto gt by the similarity transform with a
+ *                                                            proper rotation (VideoPose3D's p_mpjpe: SVD, det(R) = -1 sign fix)
+ *   acc[e, 3] += mean |d_t[j] - d_{t-1}[j]|        (t >= 1)  vel_dist   = |(p_t - p_{t-1}) - (g_t - g_{t-1})|
+ *   acc[e, 4] += mean |d_t - 2 d_{t-1} + d_{t-2}|  (t >= 2)  accel_dist
+ *   acc[e, 5..7] += 1 for the frames counted in 0-2, 3 and 4.
+ * Sums are in the units of the positions (metres; compute_metrics_lite reports millimetres), fp64, added in a fixed order (no
+ * atomics): bit-identical from run to run.  d_t is written to ring[t & 1] on every step; ring[(t + 1) & 1] must hold d_{t-1} for
+ * t >= 1 and ring[t & 1] d_{t-2} for t >= 2, i.e. call once per step with t = 0, 1, 2, ... (t restarts at 0 for a new batch of
+ * clips, the ring needs no reset).  body_pos: element (e, j, c) at e * env_stride + j * body_stride + c * coord_stride floats
+ * (coord_stride must be 1; e.g. the [..., :J, 0:3] view of the [N, B, 13] rigid-body state); body_pos_gt [n, J, 3] contiguous;
+ * num_steps [n] int32 (get_motion_num_steps()); ring [2, n, J, 3] fp32; acc [n, PHC_EVAL_ACC_FIELDS] fp64.  1 <= J <= 64, n >= 1. */
+#define PHC_EVAL_ACC_FIELDS 8
+PHC_API int phc_eval_metrics_step(const float* body_pos, int64_t env_stride, int64_t body_stride, int64_t coord_stride,
+                                  const float* body_pos_gt, const int32_t* num_steps, int32_t t, int64_t n, int32_t num_bodies,
+                                  float* ring, double* acc, void* stream);
+
 /* build_amp_obs_demo (humanoid_amp.py:253-284) and the history re-initialisation of _init_amp_obs_ref
  * (:575-603): AMP observations of the REFERENCE motion at t0 - (first_step + k)*dt, k = 0..num_steps-1,
  * written to out[n, num_steps, A] (row stride out_stride floats).  Needs lib->frames_joint. */

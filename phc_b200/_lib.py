@@ -34,6 +34,7 @@ PHC_MAX_BODIES = 64
 PHC_LANE_BODIES = 32
 PHC_MAX_AMP_JOINTS = 64
 PHC_MAX_EXT_BODIES = 8
+PHC_EVAL_ACC_FIELDS = 8
 
 _p = C.c_void_p
 
@@ -131,6 +132,7 @@ SIGNATURES = {
     "phc_getup_reset": (C.c_int, [_p, _p, _p, _p, _p, _p, _p, C.c_int32, _p, _p, C.c_int64, _p, _p, _p, C.c_int64, _p, C.c_int32, _p,
                                   C.c_int32, _p, _p, _p, _p, _p, _p]),
     "phc_amp_ring_fill": (C.c_int, [_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _p, _p, _p]),
+    "phc_eval_metrics_step": (C.c_int, [_p, C.c_int64, C.c_int64, C.c_int64, _p, _p, C.c_int32, C.c_int64, C.c_int32, _p, _p, _p]),
     "phc_gae": (C.c_int, [_p, _p, _p, _p, C.c_int32, C.c_int64, C.c_float, C.c_float, _p, _p, _p]),
     "phc_adv_norm_workspace_bytes": (C.c_int64, [C.c_int64]),
     "phc_adv_norm": (C.c_int, [_p, _p, C.c_int64, C.c_int32, _p, _p, _p]),

@@ -31,6 +31,7 @@ SOURCES = {
     "env_step_fast.cu": [],
     "env_step_wide.cu": [],
     "getup.cu": [],
+    "eval_metrics.cu": [],
     "motion.cu": ["-fmad=false"],
     "motion_wide.cu": ["-fmad=false"],
     "motion_load.cu": ["-fmad=false"],

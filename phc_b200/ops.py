@@ -585,6 +585,34 @@ def amp_ring_fill(ring: torch.Tensor, head, mask: torch.Tensor) -> None:
     _lib.check(lib.phc_amp_ring_fill(ring.data_ptr(), ring.stride(0), n, S, A, _ptr(head), mask.data_ptr(), _stream()), "phc_amp_ring_fill")
 
 
+def eval_metrics_step(body_pos: torch.Tensor, body_pos_gt: torch.Tensor, num_steps: torch.Tensor, t: int, ring: torch.Tensor,
+                      acc: torch.Tensor) -> None:
+    """phc_eval_metrics_step: adds eval step `t`'s frame to the per-env metric sums `acc` [N, 8] fp64 (mpjpe_g, mpjpe_l, mpjpe_pa,
+    vel_dist, accel_dist in metres, then three frame counts) -- the per-step part of compute_metrics_lite over the reference's clip
+    slices (im_amp.py:244-363).  body_pos: [N, J, 3] fp32, any env / body strides with x, y, z contiguous (the `[..., :J, 0:3]` view
+    of the rigid-body state); body_pos_gt [N, J, 3]; num_steps [N] int32; ring [2, N, J, 3] fp32 (d_{t-1}, d_{t-2})."""
+    if body_pos.dim() != 3 or body_pos.shape[-1] != 3:
+        raise ValueError(f"body_pos: expected [N, J, 3], got {tuple(body_pos.shape)}")
+    n, J = int(body_pos.shape[0]), int(body_pos.shape[1])
+    if not 1 <= J <= 64:
+        raise ValueError(f"eval_metrics_step: J = {J} bodies, the kernel takes 1..64")
+    if not body_pos.is_cuda:
+        raise PhcError(f"body_pos: phc_b200 runs on CUDA tensors only (got {body_pos.device}); there is no CPU fallback")
+    if body_pos.dtype != torch.float32 or body_pos.stride(-1) != 1:
+        raise ValueError("body_pos: fp32 with x, y, z contiguous")
+    dev = body_pos.device
+    _req(body_pos_gt, torch.float32, "body_pos_gt", dev)
+    _req(num_steps, torch.int32, "num_steps", dev)
+    _req(ring, torch.float32, "ring", dev)
+    _req(acc, torch.float64, "acc", dev)
+    assert body_pos_gt.shape == (n, J, 3) and num_steps.shape == (n,) and ring.shape == (2, n, J, 3)
+    assert acc.shape == (n, _lib.PHC_EVAL_ACC_FIELDS)
+    lib = _lib.load()
+    _lib.check(lib.phc_eval_metrics_step(body_pos.data_ptr(), body_pos.stride(0), body_pos.stride(1), body_pos.stride(2),
+                                         body_pos_gt.data_ptr(), num_steps.data_ptr(), int(t), n, J, ring.data_ptr(), acc.data_ptr(),
+                                         _stream()), "phc_eval_metrics_step")
+
+
 def amp_window_export(ring: torch.Tensor, head, out: torch.Tensor) -> torch.Tensor:
     """out[n, k, :] = ring[n, (head + k) % S, :] -- newest-first AMP window from the ring (phc_amp_window_export).
     `head`: an int, or the int32 [1] device tensor that holds it."""
