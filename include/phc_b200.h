@@ -365,6 +365,18 @@ PHC_API int phc_eval_metrics_step(const float* body_pos, int64_t env_stride, int
                                   const float* body_pos_gt, const int32_t* num_steps, int32_t t, int64_t n, int32_t num_bodies,
                                   float* ring, double* acc, void* stream);
 
+/* ------------------------------------------------------------------------------------------------------------
+ * Episode statistics of the rollout: the per-step bookkeeping of AMPAgent.play_steps (phc/learning/amp_agent.py:358-369) with
+ * rl_games 1.1.4's AverageMeter, ONE launch per step, no host sync.  For every env i (dones: the int64 reset flags):
+ *   v_r = cur_r[i] + rewards[i], v_l = cur_l[i] + 1; cur_r[i] = v_r * (1 - done), cur_l[i] = v_l * (1 - done)   (fp32)
+ * and, when k = #(done != 0) > 0, the meters m = 0 (game_rewards, values v_r) and m = 1 (game_lengths, values v_l) of the done envs:
+ *   new_mean = mean of the k values; size = min(k, games_to_track); old = min(games_to_track - size, meter_size[m])
+ *   meter_mean[m] = (meter_mean[m] * old + new_mean * size) / (old + size); meter_size[m] = old + size
+ * rewards, cur_r, cur_l [n] fp32; dones [n] int64; meter_mean [2] fp32; meter_size [2] int32.  Fixed-order sums (fp64), no
+ * atomics: bit-identical from run to run.  n >= 1, games_to_track >= 1. */
+PHC_API int phc_episode_stats(const float* rewards, const int64_t* dones, int64_t n, float* cur_r, float* cur_l, float* meter_mean,
+                              int32_t* meter_size, int32_t games_to_track, void* stream);
+
 /* build_amp_obs_demo (humanoid_amp.py:253-284) and the history re-initialisation of _init_amp_obs_ref
  * (:575-603): AMP observations of the REFERENCE motion at t0 - (first_step + k)*dt, k = 0..num_steps-1,
  * written to out[n, num_steps, A] (row stride out_stride floats).  Needs lib->frames_joint. */
@@ -584,7 +596,8 @@ PHC_API int phc_ppo_grads_gather(const float* mu, int64_t ldmu, const float* log
                          float* dmu, int64_t lddmu, float* dv, int64_t lddv, float* stats, void* stream);
 /* AMPAgent._disc_loss prediction part (amp_agent.py:739-743, :791-804): rows [0,n_agent) are agent+replay logits
  * (target 0), rows [n_agent, n_agent+n_demo) demo logits (target 1); dlogit = coef*0.5*dBCE/n.
- * stats[6] += sum softplus(agent) [7] += sum softplus(-demo) [8] += #(agent<0) [9] += #(demo>0) */
+ * stats[6] += sum softplus(agent) [7] += sum softplus(-demo) [8] += #(agent<0) [9] += #(demo>0)
+ * [13] += sum agent logit [14] += sum demo logit (stats must hold at least 15 floats) */
 PHC_API int phc_disc_logit_grad(const float* logit, int64_t ld, int64_t n_agent, int64_t n_demo, float coef, float* dlogit,
                         int64_t ldd, float* stats, void* stream);
 /* AMPAgent._calc_disc_rewards (:864-878) (+ _combine_rewards :848-853 when combined != NULL) */

@@ -133,6 +133,7 @@ SIGNATURES = {
                                   C.c_int32, _p, _p, _p, _p, _p, _p]),
     "phc_amp_ring_fill": (C.c_int, [_p, C.c_int64, C.c_int64, C.c_int32, C.c_int32, _p, _p, _p]),
     "phc_eval_metrics_step": (C.c_int, [_p, C.c_int64, C.c_int64, C.c_int64, _p, _p, C.c_int32, C.c_int64, C.c_int32, _p, _p, _p]),
+    "phc_episode_stats": (C.c_int, [_p, _p, C.c_int64, _p, _p, _p, _p, C.c_int32, _p]),
     "phc_gae": (C.c_int, [_p, _p, _p, _p, C.c_int32, C.c_int64, C.c_float, C.c_float, _p, _p, _p]),
     "phc_adv_norm_workspace_bytes": (C.c_int64, [C.c_int64]),
     "phc_adv_norm": (C.c_int, [_p, _p, C.c_int64, C.c_int32, _p, _p, _p]),

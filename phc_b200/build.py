@@ -32,6 +32,7 @@ SOURCES = {
     "env_step_wide.cu": [],
     "getup.cu": [],
     "eval_metrics.cu": [],
+    "episode_stats.cu": [],
     "motion.cu": ["-fmad=false"],
     "motion_wide.cu": ["-fmad=false"],
     "motion_load.cu": ["-fmad=false"],

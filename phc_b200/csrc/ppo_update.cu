@@ -34,8 +34,9 @@ __device__ __forceinline__ double wsumd(double v) {
 // (a ticket, as in colsum_group_kernel) adds the partials of all blocks -- thread t the blocks t, t + blockDim.x, ... in order, then
 // the warps in order -- into out[0 .. K).  The sums do not depend on which block finishes first, so they repeat bit for bit.
 // Launches rotate through STAT_SLOTS partial buffers and tickets (the kernels' `slot` argument), so that launches in flight on
-// different streams never share one.
-constexpr int STAT_SLOTS = 8, STAT_MAX_BLOCKS = 132 * 8, STAT_MAX_K = 5;
+// different streams never share one.  Statistic k goes to out[k] for k < SPLIT and to out[k + GAP] from SPLIT on (a kernel whose
+// later statistics live in slots further along the caller's buffer).
+constexpr int STAT_SLOTS = 8, STAT_MAX_BLOCKS = 132 * 8, STAT_MAX_K = 6;
 __device__ float g_stat_parts[STAT_SLOTS][STAT_MAX_BLOCKS * STAT_MAX_K];
 __device__ unsigned int g_stat_tickets[STAT_SLOTS];      // blocks of the launch done so far (zero between launches)
 
@@ -50,7 +51,7 @@ __device__ unsigned int g_stat_tickets[STAT_SLOTS];      // blocks of the launch
 #endif
 
 // blk[0 .. K): this block's totals in shared memory, complete for every thread; blockDim.x is a multiple of 32, gridDim.x <= STAT_MAX_BLOCKS
-template <int K>
+template <int K, int SPLIT = K, int GAP = 0>
 __device__ void stats_fixed_order(const float* blk, float* __restrict__ out, unsigned int slot) {
   __shared__ bool last;
   __shared__ float wpart[32];
@@ -75,7 +76,7 @@ __device__ void stats_fixed_order(const float* blk, float* __restrict__ out, uns
     if (threadIdx.x == 0) {
       float s = 0.f;
       for (int i = 0; i < (int)(blockDim.x >> 5); ++i) s += wpart[i];
-      out[k] += s;
+      out[k < SPLIT ? k : k + GAP] += s;
     }
     __syncthreads();
   }
@@ -425,10 +426,11 @@ __global__ void ppo_critic_grad_kernel(const float* __restrict__ v, int64_t ldv,
 
 // discriminator prediction loss: BCE-with-logits against 0 (agent + replay rows) / 1 (demo rows), 0.5 * (neg + pos)
 // dl = coef * 0.5 * dBCE/dlogit / rows.  stats[6] += sum softplus(x) agent, [7] += sum softplus(-x) demo,
-// [8] += #(agent logit < 0), [9] += #(demo logit > 0)
+// [8] += #(agent logit < 0), [9] += #(demo logit > 0), [13] += sum agent logit, [14] += sum demo logit
+// (slots 10-12 belong to the gradient penalty and the regularisers)
 __global__ void disc_logit_grad_kernel(const float* __restrict__ logit, int64_t ld, int64_t n_agent, int64_t n_demo,
                                        float coef, float* __restrict__ dlogit, int64_t ldd, float* __restrict__ stats, unsigned int slot = 0) {
-  float la = 0.f, lp = 0.f, ca = 0.f, cd = 0.f;
+  float la = 0.f, lp = 0.f, ca = 0.f, cd = 0.f, xa = 0.f, xd = 0.f;
   const int64_t n = n_agent + n_demo;
   for (int64_t i = (int64_t)blockIdx.x * blockDim.x + threadIdx.x; i < n; i += (int64_t)gridDim.x * blockDim.x) {
     const float x = logit[i * ld];
@@ -437,17 +439,19 @@ __global__ void disc_logit_grad_kernel(const float* __restrict__ logit, int64_t 
     if (i < n_agent) {
       la += sp;
       ca += (x < 0.f) ? 1.f : 0.f;
+      xa += x;
       dlogit[i * ldd] = coef * 0.5f * sig / (float)n_agent;
     } else {
       lp += sp - x;                                                    // softplus(-x)
       cd += (x > 0.f) ? 1.f : 0.f;
+      xd += x;
       dlogit[i * ldd] = coef * 0.5f * (sig - 1.0f) / (float)n_demo;
     }
   }
-  float v[4] = {la, lp, ca, cd};
-  __shared__ float blk[4];
-  block_totals<4>(v, blk);
-  stats_fixed_order<4>(blk, stats + 6, slot);
+  float v[6] = {la, lp, ca, cd, xa, xd};
+  __shared__ float blk[6];
+  block_totals<6>(v, blk);
+  stats_fixed_order<6, 4, 3>(blk, stats + 6, slot);
 }
 
 // disc reward (amp_agent.py:864-878) fused with _combine_rewards (:848-853):

@@ -16,6 +16,7 @@ from __future__ import annotations
 
 import copy
 import os
+import sys
 import time
 from typing import Dict, Optional
 
@@ -153,6 +154,25 @@ class RunningMeanStd:
         self.count.copy_(sd["count"].to(self.device))
 
 
+class DeviceAverageMeter:
+    """rl_games 1.1.4 torch_ext.AverageMeter (max_size = games_to_track) kept on the device: `mean` is a [1] fp32 view and `size` a [1]
+    int32 view into the buffers that phc_episode_stats updates inside the rollout (graph), so reading them is a host sync."""
+
+    def __init__(self, mean: torch.Tensor, size: torch.Tensor, max_size: int):
+        self.mean, self.size, self.max_size = mean, size, int(max_size)
+
+    @property
+    def current_size(self) -> int:
+        return int(self.size.item())
+
+    def get_mean(self) -> torch.Tensor:
+        return self.mean
+
+    def clear(self) -> None:
+        self.mean.zero_()
+        self.size.zero_()
+
+
 class ReplayBuffer:
     """phc/learning/replay_buffer.py with index-returning sampling (rows are gathered later, once, by the consumer)."""
 
@@ -235,6 +255,9 @@ class AMPAgent:
         self._disc_reward_scale = float(cfg["disc_reward_scale"])
         self._normalize_amp_input = bool(cfg["normalize_amp_input"])
         self._amp_replay_keep_prob = float(cfg["amp_replay_keep_prob"])
+        self.games_to_track = int(cfg.get("games_to_track", 100))
+        if self.games_to_track < 1:
+            raise ValueError(f"AMPAgent: games_to_track = {self.games_to_track}, must be >= 1")
         self.temp_running_mean = getattr(task, "temp_running_mean", True)
 
         self.obs_dim = task.get_obs_size()
@@ -387,13 +410,22 @@ class AMPAgent:
         self._gp_u = [z(Bd, round4(l.out_dim)) for l in du]
         self._gp_e = [z(Bd, round4(l.out_dim)) for l in du]
         self._gp_g = z(Bd, self.amp_pad)
-        self._stats = z(16)
+        # loss statistics, one row of 16 per minibatch of the epoch (train_result_dict reads the last one).  Slots: 0 actor loss,
+        # 1 bound loss, 2 #clipped, 3 kl, 4 entropy, 5 critic loss, 6/7 disc BCE agent/demo, 8/9 disc hits agent/demo,
+        # 10 grad penalty, 11 logit regulariser, 12 sum of squared disc weights, 13/14 sum of agent/demo logits (sums over rows)
+        self._epoch_stats = z(self.mini_epochs_num * self.num_minibatches, 16)
+        self._stats = self._epoch_stats[0]
+        self._stat_div = torch.tensor([B] * 6 + [2 * Bd, Bd, 2 * Bd, Bd, Bd, 1, 1, 2 * Bd, Bd], dtype=torch.float64, device=dev)
         # disc reward over the whole rollout, evaluated in chunks of the amp update batch
         self._ws_disc_r = self.engine.workspace("disc_r", self.model.disc, 3 * Bd)
         self._no_dones = torch.zeros(N, dtype=torch.int64, device=dev)
-        self.game_rewards = z(N)
         self.current_rewards = z(N)
         self.current_lengths = z(N)
+        # game_rewards / game_lengths meters: [rewards, lengths] means and sizes, updated by phc_episode_stats every rollout step
+        self._meter_mean = z(2)
+        self._meter_size = torch.zeros(2, dtype=torch.int32, device=dev)
+        self.game_rewards = DeviceAverageMeter(self._meter_mean[0:1], self._meter_size[0:1], self.games_to_track)
+        self.game_lengths = DeviceAverageMeter(self._meter_mean[1:2], self._meter_size[1:2], self.games_to_track)
 
     # ------------------------------------------------------------------------------------------------------
     # observation / value pre-processing
@@ -566,9 +598,10 @@ class AMPAgent:
                     next_vals = self._eval_critic(self.obs)
                     next_vals *= (1.0 - terminated.unsqueeze(-1))
                     eb["next_values"][n].copy_(next_vals)
-            not_dones = 1.0 - self.dones.float()
-            self.current_rewards.add_(rewards.squeeze(1)).mul_(not_dones)      # in place: state carried across (graph-replayed) rollouts
-            self.current_lengths.add_(1).mul_(not_dones)
+            # returns / lengths of the episodes that ended into the meters, then zeroed where done (in place: state carried across
+            # graph-replayed rollouts)
+            ops.episode_stats(rewards.view(-1), self.dones, self.current_rewards, self.current_lengths, self._meter_mean, self._meter_size,
+                              self.games_to_track)
             done_mask = self.dones
 
         if self._defer_critic:
@@ -719,7 +752,10 @@ class AMPAgent:
         it = indices()
         idx = next(it, None)
         prepared = self._prepare_minibatch(idx) if (grouped and idx is not None) else None
+        row = 0
         while idx is not None:
+            self._stats = self._epoch_stats[row]           # this minibatch's row of the loss statistics
+            row += 1
             self._compute_gradients(idx, prepared)
             scale = self._reducer.begin(self.model.grads) if self.multi_gpu else 1.0
             idx = next(it, None)                       # (a new permutation is drawn here at mini-epoch boundaries)
@@ -919,6 +955,17 @@ class AMPAgent:
                     disc_agent_acc=s[8] / (2 * Bd), disc_demo_acc=s[9] / Bd, disc_grad_penalty=s[10] / Bd,
                     disc_logit_loss=s[11])
 
+    # the per-minibatch scalars of train_result_dict as stats-row / divisor, slot by slot, then slot 12 (sum of squared disc weights)
+    # and the mean agent / demo logits of slots 13 / 14
+    _STAT_KEYS = ("actor_loss", "b_loss", "actor_clip_frac", "kl", "entropy", "critic_loss", "disc_loss_agent", "disc_loss_demo",
+                  "disc_agent_acc", "disc_demo_acc", "disc_grad_penalty", "disc_logit_loss", "disc_weight_sumsq", "disc_agent_logit",
+                  "disc_demo_logit")
+
+    def _epoch_stat_means(self) -> torch.Tensor:
+        """[15] fp64 on the device: every _STAT_KEYS scalar averaged over the epoch's minibatches (torch_ext.mean_list of the
+        reference's per-minibatch train_info); no host sync."""
+        return (self._epoch_stats[:, :15].double() / self._stat_div).mean(0)
+
     def _disc_loss(self, disc_agent_logit=None, disc_demo_logit=None, obs_demo=None) -> Dict[str, float]:
         """AMPAgent._disc_loss (amp_agent.py:732-789).  The loss and its gradient (incl. the gradient penalty) are produced
         inside calc_gradients by phc_disc_logit_grad + the GEMM chain; this returns the reference's info dict for the LAST
@@ -1005,17 +1052,131 @@ class AMPAgent:
         self.frame += self.batch_size * self.world
         return dict(play_time=t1 - t0, update_time=t2 - t1, total_time=t2 - t0, terminated_flags=batch_dict["terminated_flags"],
                     reward_raw=batch_dict["reward_raw"], mb_rewards=batch_dict["mb_rewards"], returns=batch_dict["returns"],
-                    disc_rewards=batch_dict["disc_rewards"])
+                    disc_rewards=batch_dict["disc_rewards"], last_lr=self.last_lr, lr_mul=1.0,
+                    # the epoch's statistics, kept out of the top level so that the tensors a caller gets back stay the ones above
+                    epoch_stats={"loss_means": self._epoch_stat_means()})
 
     def train(self, max_epochs: Optional[int] = None):
-        """CommonAgent.train (common_agent.py:100-185) without the logging / checkpoint cadence side channels."""
+        """CommonAgent.train (common_agent.py:100-185).  When the config carries `network_path` (run_hydra.py sets it), the reference's
+        checkpoint / evaluation / logging cadence runs around the epochs (_train_with_cadence); without it only the epochs run and
+        nothing is written.  Returns the last epoch's train_epoch() dict."""
         self.obs = self.env_reset()
         self._init_amp_demo_buf()
         max_epochs = self.config["max_epochs"] if max_epochs is None else max_epochs
+        if self.config.get("network_path") is not None:
+            return self._train_with_cadence(int(max_epochs))
         info = None
         while self.epoch_num < max_epochs:
             info = self.train_epoch()
         return info
+
+    def _train_with_cadence(self, max_epochs: int):
+        """The loop of CommonAgent.train with the reference's epoch numbering (self.epoch_num after train_epoch):
+        `<network_path>/<name>.pth` every min(50, save_best_after) epochs; with save_intermediate `<name>_<epoch:08d>.pth` every
+        save_frequency epochs and, when episodes have finished, eval() there (has_eval); a final save once epoch > max_epochs.
+        Per epoch ONE packed device->host read feeds the scalars.  Only rank 0 writes, saves and evaluates."""
+        cfg = self.config
+        network_path = cfg["network_path"]
+        model_output_file = os.path.join(network_path, cfg["name"])
+        save_freq, save_best_after = int(cfg["save_frequency"]), int(cfg["save_best_after"])
+        save_intermediate, has_eval = bool(cfg.get("save_intermediate", False)), bool(cfg.get("has_eval", True))
+        exp_name = os.path.basename(os.path.normpath(cfg.get("train_dir", network_path)))
+        if self.rank == 0:
+            os.makedirs(network_path, exist_ok=True)
+            self.writer = cfg.get("writer") or self._make_writer(os.path.join(network_path, "summaries"))
+        total_time = 0.0
+        info = None
+        while True:
+            epoch_start = time.time()
+            info = self.train_epoch()
+            epoch_num = self.epoch_num
+            total_time += info["total_time"]
+            if self.rank != 0:
+                if epoch_num > max_epochs:
+                    return info
+                continue
+            host = self._read_epoch_scalars(info)               # the one device->host read of the epoch
+            frame = self.frame - self.batch_size * self.world   # frames before this epoch, as the reference logs them
+            curr_frames = self.batch_size * self.world
+            fps_step, fps_total = curr_frames / max(info["play_time"], 1e-9), curr_frames / max(info["total_time"], 1e-9)
+            self.writer.add_scalar("performance/total_fps", fps_total, frame)
+            self.writer.add_scalar("performance/step_fps", fps_step, frame)
+            self.writer.add_scalar("episode_lengths/epochs", epoch_num, frame)
+            train_info_dict = self._assemble_train_info(info, frame)
+            intermediate = save_intermediate and save_freq > 0 and epoch_num % save_freq == 0
+            if save_freq > 0:
+                if epoch_num % min(50, save_best_after) == 0:
+                    self.save(model_output_file)
+                if intermediate:
+                    self.save(model_output_file + "_" + str(epoch_num).zfill(8))
+            if host["game_size"] > 0:
+                mean_rewards, mean_lengths = host["game_rewards"], host["game_lengths"]
+                self.writer.add_scalar("rewards0/frame", mean_rewards, frame)
+                self.writer.add_scalar("rewards0/iter", mean_rewards, epoch_num)
+                self.writer.add_scalar("rewards0/time", mean_rewards, total_time)
+                self.writer.add_scalar("episode_lengths/frame", mean_lengths, frame)
+                self.writer.add_scalar("episode_lengths/iter", mean_lengths, epoch_num)
+                if intermediate and has_eval:
+                    train_info_dict.update(self.eval())
+                train_info_dict.update({"episode_lengths/episode_lengths": mean_lengths, "rewards/mean_rewards": mean_rewards})
+                self._log_train_info(train_info_dict, frame)
+                print(f"{exp_name}-Ep: {self.epoch_num}\trwd: {mean_rewards:.1f}\tfps_step: {fps_step:.1f}\tfps_total: {fps_total:.1f}"
+                      f"\tep_time:{time.time() - epoch_start:.1f}\tframe: {self.frame}\teps_len: {mean_lengths:.1f}")
+            if epoch_num > max_epochs:
+                self.save(model_output_file)
+                print("MAX EPOCHS NUM!")
+                return info
+
+    @staticmethod
+    def _make_writer(log_dir: str):
+        from torch.utils.tensorboard import SummaryWriter
+        return SummaryWriter(log_dir)
+
+    def _read_epoch_scalars(self, train_info) -> Dict[str, float]:
+        """Everything the epoch's log needs, packed on the device and read back at once: the loss means (_STAT_KEYS), the meters,
+        the means of returns / mb_rewards, the disc reward's std and mean and the reward_raw components.  Stored in
+        train_info["host"]."""
+        reward_raw = train_info["reward_raw"].reshape(-1)
+        disc_std, disc_mean = torch.std_mean(train_info["disc_rewards"])
+        parts = [train_info["epoch_stats"]["loss_means"], self._meter_mean, self._meter_size[:1], train_info["returns"].mean().reshape(1),
+                 train_info["mb_rewards"].mean().reshape(1), disc_std.reshape(1), disc_mean.reshape(1), reward_raw]
+        v = torch.cat([p.double().reshape(-1) for p in parts]).tolist()
+        nk = len(self._STAT_KEYS)
+        host = dict(zip(self._STAT_KEYS, v[:nk]))
+        host.update(game_rewards=v[nk], game_lengths=v[nk + 1], game_size=int(v[nk + 2]), returns=v[nk + 3], mb_rewards=v[nk + 4],
+                    disc_reward_std=v[nk + 5], disc_reward_mean=v[nk + 6], reward_raw=v[nk + 7:])
+        train_info["host"] = host
+        return host
+
+    def _assemble_train_info(self, train_info, frame) -> Dict[str, float]:
+        """CommonAgent._assemble_train_info + AMPAgent._assemble_train_info (common_agent.py:604-625, amp_agent.py:901-937) from the
+        host scalars of _read_epoch_scalars: losses and discriminator statistics are means over the epoch's minibatches."""
+        h = train_info["host"] if "host" in train_info else self._read_epoch_scalars(train_info)
+        lr_mul = train_info.get("lr_mul", 1.0)
+        d = {"performance/update_time": train_info["update_time"], "performance/play_time": train_info["play_time"],
+             "learning_rate/last_lr": train_info.get("last_lr", self.last_lr) * lr_mul, "learning_rate/lr_mul": lr_mul,
+             "learning_rate/e_clip": self.e_clip * lr_mul,
+             "loss/actor_loss": h["actor_loss"], "loss/critic_loss": h["critic_loss"], "loss/bounds_loss": h["b_loss"],
+             "loss/entropy": h["entropy"], "loss/clip_frac": h["actor_clip_frac"], "loss/kl": h["kl"]}
+        disc_loss = (0.5 * (h["disc_loss_agent"] + h["disc_loss_demo"]) + self._disc_logit_reg * h["disc_logit_loss"]
+                     + self._disc_grad_penalty * h["disc_grad_penalty"] + self._disc_weight_decay * h["disc_weight_sumsq"])
+        d.update({"disc/loss": disc_loss, "disc/agent_acc": h["disc_agent_acc"], "disc/demo_acc": h["disc_demo_acc"],
+                  "disc/agent_logit": h["disc_agent_logit"], "disc/demo_logit": h["disc_demo_logit"],
+                  "disc/grad_penalty": h["disc_grad_penalty"], "disc/logit_loss": h["disc_logit_loss"],
+                  "disc/reward_mean": h["disc_reward_mean"], "disc/reward_std": h["disc_reward_std"],
+                  "rewards/returns": h["returns"], "rewards/mb_rewards": h["mb_rewards"]})
+        for k, v in zip(("body_pos", "body_rot", "lin_vel", "ang_vel", "power"), h["reward_raw"]):
+            d["rewards/" + k] = v
+        return d
+
+    def _log_train_info(self, train_info, frame) -> None:
+        """CommonAgent._log_train_info (common_agent.py:627-635): every scalar to the writer at step epoch_num, and to wandb when a
+        wandb run is active (a run can only be active when the user's script imported wandb)."""
+        for k, v in train_info.items():
+            self.writer.add_scalar(k, v, self.epoch_num)
+        wandb = sys.modules.get("wandb")
+        if wandb is not None and getattr(wandb, "run", None) is not None:
+            wandb.log(train_info, step=self.epoch_num)
 
     # ------------------------------------------------------------------------------------------------------
     # checkpoint dict, same keys as the reference (amp_agent.py:69-102,:158-166; SURVEY.md section 5)

@@ -18,6 +18,7 @@ long clips weigh more, `succ` falling back to `all` when no clip succeeded, NaN 
 """
 from __future__ import annotations
 
+import glob
 import os
 from typing import Dict, List, Tuple
 
@@ -45,6 +46,20 @@ class IMAmpAgent(AMPAgent):
     def env_eval_step(self, env, actions):
         obs, rewards, dones, infos = env.step(actions)
         return obs, rewards, dones, infos
+
+    # ---- im_amp.py:101-117 -----------------------------------------------------------------------------------------
+    def restore(self, fn: str) -> None:
+        """AMPAgent.restore, then the Auto-PMCP termination history of the newest `<network_path>/failed_*.pkl` (update_training_data
+        writes one per evaluation) back into the motion sampling weights, so a resumed run keeps them."""
+        super().restore(fn)
+        fails = glob.glob(os.path.join(self.network_path, "failed_*"))
+        if not fails:
+            return
+        newest = sorted(fails, key=lambda x: int(x.split("_")[-1].split(".")[0]))[-1]
+        import joblib
+        termination_history = joblib.load(newest)["termination_history"]
+        ok = self.vec_env.env.task._motion_data.update_sampling_prob(termination_history)
+        print(f"restored the termination history of {newest}" if ok else f"{newest}: termination history length does not match")
 
     # ---- im_amp.py:124-133 -----------------------------------------------------------------------------------------
     def update_training_data(self, failed_keys) -> None:

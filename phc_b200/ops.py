@@ -613,6 +613,27 @@ def eval_metrics_step(body_pos: torch.Tensor, body_pos_gt: torch.Tensor, num_ste
                                          _stream()), "phc_eval_metrics_step")
 
 
+def episode_stats(rewards: torch.Tensor, dones: torch.Tensor, cur_r: torch.Tensor, cur_l: torch.Tensor, meter_mean: torch.Tensor,
+                  meter_size: torch.Tensor, games_to_track: int) -> None:
+    """phc_episode_stats: one rollout step of the episode bookkeeping (amp_agent.py:358-369).  cur_r += rewards and cur_l += 1, the
+    returns and lengths of the envs with dones != 0 are folded into the meters (rl_games' AverageMeter.update, max_size =
+    games_to_track), then both are zeroed where done.  rewards, cur_r, cur_l [N] fp32; dones [N] int64 (reset_buf);
+    meter_mean [2] fp32 and meter_size [2] int32: game_rewards, game_lengths."""
+    dev = cur_r.device
+    _req(rewards, torch.float32, "rewards", dev)
+    _req(dones, torch.int64, "dones", dev)
+    _req(cur_r, torch.float32, "cur_r", dev)
+    _req(cur_l, torch.float32, "cur_l", dev)
+    _req(meter_mean, torch.float32, "meter_mean", dev)
+    _req(meter_size, torch.int32, "meter_size", dev)
+    n = cur_r.numel()
+    if rewards.numel() != n or dones.numel() != n or cur_l.numel() != n or meter_mean.numel() != 2 or meter_size.numel() != 2:
+        raise ValueError("episode_stats: rewards, dones, cur_r, cur_l must have N elements, meter_mean and meter_size 2")
+    lib = _lib.load()
+    _lib.check(lib.phc_episode_stats(rewards.data_ptr(), dones.data_ptr(), n, cur_r.data_ptr(), cur_l.data_ptr(), meter_mean.data_ptr(),
+                                     meter_size.data_ptr(), int(games_to_track), _stream()), "phc_episode_stats")
+
+
 def amp_window_export(ring: torch.Tensor, head, out: torch.Tensor) -> torch.Tensor:
     """out[n, k, :] = ring[n, (head + k) % S, :] -- newest-first AMP window from the ring (phc_amp_window_export).
     `head`: an int, or the int32 [1] device tensor that holds it."""
