@@ -497,6 +497,11 @@ typedef struct PhcGemmDesc {
                              * by bulk copy and never looks at a_kmajor / b_kmajor; the result is again the same bit for bit, and
                              * the same two cases ignore both images.  Meant for the weight gradient (dW += dY^T X, both operands
                              * mn-major activations), whose images are made once per launch instead of staged once per tile. */
+  float* C_img;             /* optional: the epilogue also writes the image of the stored output with rows = M and K = N (the
+                             * layout phc_gemm_make_images makes from C with b_kmajor = 1, bit for bit, zero outside M x N), so that
+                             * the next layer's forward or input-gradient GEMM can take C as its A_img without a separate pass.
+                             * 16-byte aligned, phc_gemm_image_floats(M, N) floats.  Refused with accumulate, k_splits > 1, 128 x 256
+                             * tiles and PHC_GEMM_TF32_SINGLE_PASS. */
 } PhcGemmDesc;
 /* Weight image of a B operand (B(n,k) as in PhcGemmDesc, N x K): one block of 8192 floats per (128-row n-tile nt, 32-wide k-block
  * kb), block nt * ceil(K / 32) + kb, each block [hi | lo] of 4096 floats with hi = trunc_tf32(B), lo = rna_tf32(B - hi) (the

@@ -83,7 +83,7 @@ class PhcGemmDesc(C.Structure):
     _fields_ = [("A", _p), ("lda", C.c_int64), ("a_kmajor", C.c_int32), ("B", _p), ("ldb", C.c_int64), ("b_kmajor", C.c_int32),
                 ("C", _p), ("ldc", C.c_int64), ("M", C.c_int32), ("N", C.c_int32), ("K", C.c_int32), ("alpha", C.c_float),
                 ("bias", _p), ("act", C.c_int32), ("aux", _p), ("ldaux", C.c_int64), ("accumulate", C.c_int32), ("k_splits", C.c_int32),
-                ("B_lo", _p), ("B_img", _p), ("A_img", _p)]
+                ("B_lo", _p), ("B_img", _p), ("A_img", _p), ("C_img", _p)]
 
 
 class PhcGemmImageDesc(C.Structure):

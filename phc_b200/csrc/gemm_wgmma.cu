@@ -28,6 +28,10 @@
 // pre-split by bulk copy and A goes from global memory straight into the wgmma register fragment (the image loop below).  One
 // that also comes with an image of A (PhcGemmDesc.A_img: the weight gradient, whose operands are both mn-major activations,
 // imaged once per launch instead of once per tile) takes both operands by bulk copy into the staged loop's stages (the pair loop).
+// A problem with PhcGemmDesc.C_img (128 x 128 tiles, 3xTF32, not accumulating) also writes its output's image from the epilogue:
+// a 128 x 128 output tile is exactly four 128 x 32 image blocks, so the next layer's forward or input-gradient GEMM gets its A
+// image without a separate pass and runs on the pair loop, which keeps three k-blocks of both operands in flight and does no
+// per-thread global loads (the image loop issues 16 scalar A loads per thread and k-block, one k-block ahead).
 #include <cuda_runtime.h>
 #include <stdint.h>
 #include <stdlib.h>
@@ -72,6 +76,7 @@ struct Prob {
   const float* B_img;                                                          // weight image of B (128 x 128 tiles only), or NULL
   const float* A_img;                                                          // image of A (only with B_img), or NULL
   float* C; float* C_hi; float* C_lo;                                          // C_hi / C_lo: split copies of the result (phc_gemm_tc5)
+  float* C_img;                                                                // image of the result (rows = M, K = N), or NULL
   const float* bias;
   float* aux;
   long long lda, ldb, ldc, ldaux;
@@ -269,8 +274,11 @@ __device__ __forceinline__ void split_rna(float x, float& h, float& l) {
   h = __uint_as_float(a); l = __uint_as_float(b);
 }
 
-// SINGLE: one tensor-core product per fp32 product (plain TF32, ~1e-3 relative): no lo terms
-template <int BN, bool PRESPLIT, bool SINGLE>
+// SINGLE: one tensor-core product per fp32 product (plain TF32, ~1e-3 relative): no lo terms.  OUT_IMG: the epilogue writes
+// PhcGemmDesc.C_img where a problem has one.  It is a separate instantiation because the extra epilogue code changes how ptxas
+// schedules the whole kernel: in the one instantiation, the launches without output images ran 3-11 % slower on the bench
+// minibatch (H100 SXM, 700 W).
+template <int BN, bool PRESPLIT, bool SINGLE, bool OUT_IMG = false>
 __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid_constant__ Params P) {
   static_assert(!(PRESPLIT && SINGLE), "the pre-split operands are for the 3xTF32 products");
   using C = Cfg<BN>;
@@ -279,6 +287,7 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
   // single pass stays on the staged loop: ptxas serialises the wgmmas of its image loop (C7513)
   constexpr bool HAS_IMG = BN == IMG_ROWS && BK == IMG_BK && !PRESPLIT && !SINGLE;
   static_assert(!HAS_IMG || (C::A_TILE == IMG_HALF * 4 && C::B_TILE == IMG_HALF * 4), "an image block pair is one stage");
+  static_assert(!OUT_IMG || HAS_IMG, "output images are written by the 3xTF32 kernel with 128 x 128 tiles");
   extern __shared__ __align__(128) uint8_t smem[];
   __shared__ int s_tile;
   __shared__ __align__(8) uint64_t s_bar[IMG_STAGES];      // one mbarrier per B stage of the image loop
@@ -517,9 +526,15 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
     // ---- epilogue straight from the accumulator fragment: acc[4 j + 2 h + c] is (row w*16 + lane/4 + 8 h, col 8 j + 2 (lane%4) + c)
     const int act = q.act;
     const float* bias = (q.bias && z == 0) ? q.bias : nullptr;
+    // C_img: the stored value, split like phc_gemm_make_images, at the image position of (row m - m0 of m-tile mi, k = n); the
+    // tile's 128 rows and every 32-column k-block it starts below N are written, zeros outside M x N, so the image is the
+    // one phc_gemm_make_images would make from C.  A quad's float2 pairs of one k-block half fill 128 contiguous bytes.
+    float* cimg = nullptr;
+    if constexpr (OUT_IMG) cimg = q.C_img ? q.C_img + (long long)mi * ((q.N + IMG_BK - 1) / IMG_BK) * IMG_BLOCK : nullptr;
 #pragma unroll
     for (int h = 0; h < 2; ++h) {
-      const int m = m0 + wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;
+      const int rt = wgi * 64 + wq * 16 + (lane >> 2) + 8 * h;   // row within the tile
+      const int m = m0 + rt;
       const bool row_ok = m < q.M;
       float* crow = q.C + (long long)m * q.ldc;
       float* arow = (q.aux && act < PHC_ACT_RELU_BITS && row_ok) ? q.aux + (long long)m * q.ldaux : nullptr;
@@ -562,6 +577,12 @@ __global__ void __launch_bounds__(NUM_THREADS, 1) gemm_wgmma_kernel(const __grid
               x = silu_f(x);
             }
             v[c] = x;
+          }
+          if (OUT_IMG && cimg) {
+            const float w0 = row_ok && nb + nl < q.N ? v[0] : 0.f, w1 = row_ok && nb + nl + 1 < q.N ? v[1] : 0.f;
+            float* o = cimg + (long long)(nb >> 5) * IMG_BLOCK + 256 * (rt >> 3) + 32 * (nl >> 2) + 4 * (rt & 7) + (nl & 3);
+            *reinterpret_cast<float2*>(o) = make_float2(trunc_hi(w0), trunc_hi(w1));
+            *reinterpret_cast<float2*>(o + IMG_HALF) = make_float2(split_lo(w0), split_lo(w1));
           }
           if (!row_ok) continue;
           const int n = nb + nl;
@@ -669,12 +690,13 @@ static int num_sms() {
 
 // fills P.p[n] for one problem; returns the number of tiles it adds
 static int add_problem(Params& P, int n, int tiles, int bn, const float* A, const float* A_lo, const float* A_img, long long lda, int a_k,
-                       const float* B, const float* B_lo, const float* B_img, long long ldb, int b_k, float* Cm, float* C_hi, float* C_lo, long long ldc, int M, int N, int K,
-                       float alpha, const float* bias, int act, float* aux, long long ldaux, int accumulate, int k_splits) {
+                       const float* B, const float* B_lo, const float* B_img, long long ldb, int b_k, float* Cm, float* C_hi, float* C_lo, float* C_img,
+                       long long ldc, int M, int N, int K, float alpha, const float* bias, int act, float* aux, long long ldaux, int accumulate,
+                       int k_splits) {
   const int bk = bn == 128 ? Cfg<128>::BK : Cfg<256>::BK;
   Prob& q = P.p[n];
   q.A = A; q.A_lo = A_lo; q.B = B; q.B_lo = B_lo; q.B_img = bn == IMG_ROWS ? B_img : nullptr;
-  q.A_img = q.B_img ? A_img : nullptr; q.C = Cm; q.C_hi = C_hi; q.C_lo = C_lo; q.bias = bias; q.aux = aux;
+  q.A_img = q.B_img ? A_img : nullptr; q.C = Cm; q.C_hi = C_hi; q.C_lo = C_lo; q.C_img = C_img; q.bias = bias; q.aux = aux;
   q.lda = lda; q.ldb = ldb; q.ldc = ldc; q.ldaux = ldaux; q.M = M; q.N = N; q.K = K; q.alpha = alpha; q.act = act;
   q.accumulate = accumulate ? 1 : 0; q.a_k = a_k ? 1 : 0; q.b_k = b_k ? 1 : 0;
   int ks = k_splits < 1 ? 1 : k_splits;
@@ -691,23 +713,23 @@ static int add_problem(Params& P, int n, int tiles, int bn, const float* A, cons
   return q.tile_count;
 }
 
-template <int BN, bool PRESPLIT, bool SINGLE>
+template <int BN, bool PRESPLIT, bool SINGLE, bool OUT_IMG = false>
 static int launch_kernel(const Params& P, cudaStream_t stream) {
   static bool smem_set = false;
   if (!smem_set) {
-    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, PRESPLIT, SINGLE>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
+    cudaError_t e = cudaFuncSetAttribute(gemm_wgmma_kernel<BN, PRESPLIT, SINGLE, OUT_IMG>, cudaFuncAttributeMaxDynamicSharedMemorySize, Cfg<BN>::SMEM);
     if (e != cudaSuccess) return phc_check_cuda(e, "cudaFuncSetAttribute(gemm_wgmma)");
     smem_set = true;
   }
   const int sms = num_sms();
   const unsigned grid = (unsigned)(P.total_tiles < sms ? P.total_tiles : sms);
-  gemm_wgmma_kernel<BN, PRESPLIT, SINGLE><<<grid, NUM_THREADS, Cfg<BN>::SMEM, stream>>>(P);
+  gemm_wgmma_kernel<BN, PRESPLIT, SINGLE, OUT_IMG><<<grid, NUM_THREADS, Cfg<BN>::SMEM, stream>>>(P);
   phc_count_launches(1);
   return phc_check_cuda(cudaGetLastError(), "gemm_wgmma_kernel launch");
 }
 
 template <int BN, bool PRESPLIT>
-static int launch(Params& P, bool dynamic_sched, bool single, cudaStream_t stream) {
+static int launch(Params& P, bool dynamic_sched, bool single, cudaStream_t stream, bool out_img = false) {
   // ordered problems: split-K, or accumulating into the same C as another problem of the launch (which then shares its turnstile)
   int owner[MAX_PROBLEMS];
   bool ordered = false;
@@ -770,6 +792,8 @@ static int launch(Params& P, bool dynamic_sched, bool single, cudaStream_t strea
     P.sched = base + 2 * (launch_no++ % SCHED_SLOTS);
   }
   if constexpr (PRESPLIT) return launch_kernel<BN, true, false>(P, stream);
+  if constexpr (BN == 128)
+    if (out_img) return launch_kernel<BN, false, false, true>(P, stream);   // (validate_group: not with single pass)
   return single ? launch_kernel<BN, false, true>(P, stream) : launch_kernel<BN, false, false>(P, stream);
 }
 
@@ -793,6 +817,8 @@ static int validate_group(const PhcGemmDesc* d, int32_t count) {
     if (g.B_lo && (reinterpret_cast<uintptr_t>(g.B_lo) & 15)) { phc_set_error("phc_gemm_group: B_lo must be 16-byte aligned"); return PHC_ERR_INVALID_ARG; }
     if (g.A_img && ((reinterpret_cast<uintptr_t>(g.A_img) & 15) || !g.B_img)) { phc_set_error("phc_gemm_group: A_img must be 16-byte aligned and comes with B_img only"); return PHC_ERR_INVALID_ARG; }
     if (g.B_img && ((reinterpret_cast<uintptr_t>(g.B_img) & 15) || (!g.a_kmajor && !g.A_img))) { phc_set_error("phc_gemm_group: B_img must be 16-byte aligned and comes with a_kmajor or A_img only"); return PHC_ERR_INVALID_ARG; }
+    if (g.C_img && ((reinterpret_cast<uintptr_t>(g.C_img) & 15) || g.accumulate || ks > 1)) { phc_set_error("phc_gemm_group: C_img must be 16-byte aligned and comes without accumulate or split-K"); return PHC_ERR_INVALID_ARG; }
+    if (g.C_img && (g_tile == 256 || g_single_pass)) { phc_set_error("phc_gemm_group: C_img is written by the 3xTF32 kernel with 128 x 128 tiles only"); return PHC_ERR_UNSUPPORTED; }
   }
   // write hazards: the C spans [C, C + (M - 1) ldc + N) of two problems may only overlap when both accumulate into the same C with
   // the same shape -- they then share a turnstile and add in problem order; any other overlap would race (plain stores, or
@@ -831,10 +857,12 @@ extern "C" int phc_gemm_group(const PhcGemmDesc* d, int32_t count, void* stream)
   static Params P;      // host staging (launches are serialised by the caller's stream order; the struct is copied at launch)
   memset(&P, 0, sizeof(P));
   int tiles = 0, n = 0;
+  bool out_img = false;
   for (int i = 0; i < count; ++i) {
     const PhcGemmDesc& g = d[i];
     if (g.M == 0 || g.N == 0) continue;
-    tiles += add_problem(P, n, tiles, bn, g.A, nullptr, g.A_img, g.lda, g.a_kmajor, g.B, nullptr, g.B_img, g.ldb, g.b_kmajor, g.C, nullptr, nullptr, g.ldc,
+    out_img |= g.C_img != nullptr;
+    tiles += add_problem(P, n, tiles, bn, g.A, nullptr, g.A_img, g.lda, g.a_kmajor, g.B, nullptr, g.B_img, g.ldb, g.b_kmajor, g.C, nullptr, nullptr, g.C_img, g.ldc,
                          g.M, g.N, g.K, g.alpha, g.bias, g.act, g.aux, g.ldaux, g.accumulate, g.k_splits);
     ++n;
   }
@@ -842,7 +870,7 @@ extern "C" int phc_gemm_group(const PhcGemmDesc* d, int32_t count, void* stream)
   P.count = n; P.total_tiles = tiles;
   cudaStream_t st = static_cast<cudaStream_t>(stream);
   const bool single = g_single_pass != 0;
-  return bn == 256 ? launch<256, false>(P, g_sched == 1, single, st) : launch<128, false>(P, g_sched == 1, single, st);
+  return bn == 256 ? launch<256, false>(P, g_sched == 1, single, st) : launch<128, false>(P, g_sched == 1, single, st, out_img);
 }
 
 extern "C" int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, const float* B, int64_t ldb, int32_t b_kmajor, float* C,
@@ -851,7 +879,7 @@ extern "C" int phc_gemm_tc5s(const float* A, int64_t lda, int32_t a_kmajor, cons
   PhcGemmDesc d;
   d.A = A; d.lda = lda; d.a_kmajor = a_kmajor; d.B = B; d.ldb = ldb; d.b_kmajor = b_kmajor; d.C = C; d.ldc = ldc;
   d.M = M; d.N = N; d.K = K; d.alpha = alpha; d.bias = bias; d.act = act; d.aux = aux; d.ldaux = ldaux;
-  d.accumulate = accumulate; d.k_splits = k_splits; d.B_lo = nullptr; d.B_img = nullptr; d.A_img = nullptr;
+  d.accumulate = accumulate; d.k_splits = k_splits; d.B_lo = nullptr; d.B_img = nullptr; d.A_img = nullptr; d.C_img = nullptr;
   return phc_gemm_group(&d, 1, stream);
 }
 
@@ -872,7 +900,7 @@ extern "C" int phc_gemm_tc5(const float* A_hi, const float* A_lo, int64_t lda, i
   if ((C_hi == nullptr) != (C_lo == nullptr) || (C_hi && accumulate)) { phc_set_error("phc_gemm_tc5: C_hi/C_lo come as a pair and not with accumulate"); return PHC_ERR_INVALID_ARG; }
   static Params P;
   memset(&P, 0, sizeof(P));
-  P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, nullptr, lda, a_kmajor, B_hi, B_lo, nullptr, ldb, b_kmajor, C, C_hi, C_lo, ldc, M, N, K, alpha, bias,
+  P.total_tiles = add_problem(P, 0, 0, 128, A_hi, A_lo, nullptr, lda, a_kmajor, B_hi, B_lo, nullptr, ldb, b_kmajor, C, C_hi, C_lo, nullptr, ldc, M, N, K, alpha, bias,
                               relu, mask, ldmask, accumulate, k_splits);
   P.count = 1;
   return launch<128, true>(P, false, false, static_cast<cudaStream_t>(stream));

@@ -254,8 +254,9 @@ class MLPEngine:
         self.gemm_flops = 0.0          # algorithmic fp32 FLOPs (2 M N K) of every grouped launch so far (bench.py reads it)
         # the weight images feed the grouped 3xTF32 launches; the single-pass kernel stages B itself and never reads them
         self.uses_images = self.backend == "tc5s" and precision == "fp32"
-        # activation images of the weight-gradient operands, one buffer per (tensor, rows, K), remade by every launch that reads them
-        self._act_images: Dict[Tuple[int, int, int, int], torch.Tensor] = {}
+        # activation images, one buffer per (tensor, ld, rows, K, k-major): of the weight-gradient operands and the first layer's
+        # input (remade by every launch that reads them), and of hidden outputs (written by the epilogue of the GEMM producing them)
+        self._act_images: Dict[Tuple[int, int, int, int, bool], torch.Tensor] = {}
         if self.backend == "tc5":
             net.refresh_split()
 
@@ -324,11 +325,29 @@ class MLPEngine:
         """layer l's weight image for the forward (kmajor) or dX form, or None where the launches do not read images"""
         return self.net.image(l, kmajor) if self.uses_images else None
 
-    def gdesc(self, A, a_k, B, b_k, C, M, N, K, alpha=1.0, bias=None, act=0, aux=None, accumulate=False, k_splits=1, B_img=None):
-        """B_img: B's weight image for this N and K (AMPNetwork.image), or None to stage B from the fp32 operand."""
+    def gdesc(self, A, a_k, B, b_k, C, M, N, K, alpha=1.0, bias=None, act=0, aux=None, accumulate=False, k_splits=1, B_img=None,
+              A_img=None, C_img=None):
+        """B_img: B's weight image for this N and K (AMPNetwork.image), or None to stage B from the fp32 operand.  A_img: A's image
+        (act_image(A, M, K)); C_img: the buffer the epilogue writes C's image into (act_image(C, M, N))."""
         return _lib.PhcGemmDesc(A.data_ptr(), A.stride(0), 1 if a_k else 0, B.data_ptr(), B.stride(0), 1 if b_k else 0, C.data_ptr(),
                                 C.stride(0), M, N, K, alpha, _ptr(bias), act, _ptr(aux), aux.stride(0) if aux is not None else 0,
-                                1 if accumulate else 0, k_splits, None, _ptr(B_img))
+                                1 if accumulate else 0, k_splits, None, _ptr(B_img), _ptr(A_img), _ptr(C_img))
+
+    def act_image(self, t: torch.Tensor, rows: int, K: int, kmajor: bool = True) -> torch.Tensor:
+        """The image buffer of activation t (rows x K, k-major or mn-major), allocated on first use."""
+        key = (t.data_ptr(), t.stride(0), rows, K, kmajor)
+        img = self._act_images.get(key)
+        if img is None:
+            img = torch.empty(self.lib.phc_gemm_image_floats(rows, K), dtype=torch.float32, device=self.dev)
+            self._act_images[key] = img
+        return img
+
+    def _reads_image(self, st: MLPStack, li: int) -> bool:
+        """Whether the forward and the dX of layer li take A from its image (on the pair loop).  Hidden layers do: the GEMM that
+        produces their A writes the image from its epilogue, except the first layer's input, which run_group images once for
+        the launch.  The heads stay on the image loop: their dY comes from the loss kernels, and with N = 69 or 1 their A would
+        cost an image pass as large as the product."""
+        return self.uses_images and li < len(st.hidden)
 
     def fwd_desc(self, st: MLPStack, li: int, x: torch.Tensor, ws: Dict[str, torch.Tensor]):
         """Layer li of the forward pass of stack st on batch x / workspace ws (the same epilogues as forward())."""
@@ -343,8 +362,13 @@ class MLPEngine:
             out = ws["out"]
             act = _lib.PHC_ACT_NONE if not st.head_relu else (_lib.PHC_ACT_SILU if silu else (_lib.PHC_ACT_RELU_BITS if "obits" in ws else _lib.PHC_ACT_RELU))
             aux = None if not st.head_relu else (ws["z_out"] if silu else ws.get("obits"))
-        return self.gdesc(inp, True, net.weight(l), True, out, B, l.out_dim, l.in_dim, bias=net.bias(l), act=act, aux=aux,
-                          B_img=self.image(l, True))
+        d = self.gdesc(inp, True, net.weight(l), True, out, B, l.out_dim, l.in_dim, bias=net.bias(l), act=act, aux=aux,
+                       B_img=self.image(l, True), C_img=self.act_image(out, B, l.out_dim) if self._reads_image(st, li + 1) else None)
+        if self._reads_image(st, li) and li == 0:
+            d.image_of = (("A_img", inp, B, True),)             # made by run_group; actor and critic share the input's image
+        elif self._reads_image(st, li):
+            d.A_img = self.act_image(inp, B, l.in_dim).data_ptr()
+        return d
 
     def bwd_descs(self, st: MLPStack, li: int, x: torch.Tensor, ws: Dict[str, torch.Tensor], dx: Optional[torch.Tensor] = None):
         """(dW, dX) problems of layer li: dW[out, in] += dY^T X (split-K, reduce-add into the gradient bucket) and
@@ -356,12 +380,16 @@ class MLPEngine:
         dxd = None
         img = self.image(l, False)
         if li > 0:
+            # A = dY: the image that the dX of the layer above wrote (hidden layers); C = dh[li - 1]: its image for the dX below
+            dh = ws["dh"][li - 1]
+            imgs = dict(B_img=img, A_img=self.act_image(dY, B, l.out_dim) if self._reads_image(st, li) else None,
+                        C_img=self.act_image(dh, B, l.in_dim) if li > 1 and self._reads_image(st, li - 1) else None)
             if st.activation == "silu":
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_SILU_BWD, aux=ws["z"][li - 1], B_img=img)
+                dxd = self.gdesc(dY, True, net.weight(l), False, dh, B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_SILU_BWD, aux=ws["z"][li - 1], **imgs)
             elif "hbits" in ws:
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_MASK_BITS, aux=ws["hbits"][li - 1], B_img=img)
+                dxd = self.gdesc(dY, True, net.weight(l), False, dh, B, l.in_dim, l.out_dim, act=_lib.PHC_ACT_MASK_BITS, aux=ws["hbits"][li - 1], **imgs)
             else:
-                dxd = self.gdesc(dY, True, net.weight(l), False, ws["dh"][li - 1], B, l.in_dim, l.out_dim, aux=ws["h"][li - 1], B_img=img)
+                dxd = self.gdesc(dY, True, net.weight(l), False, dh, B, l.in_dim, l.out_dim, aux=ws["h"][li - 1], **imgs)
         elif dx is not None:
             dxd = self.gdesc(dY, True, net.weight(l), False, dx, B, l.in_dim, l.out_dim, B_img=img)
         return dw, dxd
@@ -376,28 +404,25 @@ class MLPEngine:
         # from tiles_m * tiles_n >= 4 (tiles_m + tiles_n) on.
         tm, tn = -(-M // 128), -(-N // 128)
         if self.uses_images and tm * tn >= 4 * (tm + tn):
-            d.image_of = (dY, X)
+            d.image_of = (("A_img", dY, M, False), ("B_img", X, N, False))
         return d
 
     def make_images(self, descs):
-        """Points A_img / B_img of the descriptors that ask for activation images (dw_desc) at their buffers and returns the
-        image jobs (PhcGemmImageDesc array, count), one per distinct (tensor, rows, K): actor and critic share the input's image."""
+        """Points the image fields of the descriptors that ask for activation images made before the launch (image_of: the
+        weight gradient's operands, the first layer's input) at their buffers and returns the image jobs (PhcGemmImageDesc array,
+        count), one per distinct (tensor, rows, K, order): actor and critic share the input's image."""
         jobs = {}
         for d in descs:
-            srcs = getattr(d, "image_of", None)
-            if srcs is None:
+            srcs = getattr(d, "image_of", ())
+            if not d.B_img and all(f == "A_img" for f, *_ in srcs):   # B staged from fp32 (its image cleared): so is A
+                d.A_img = None
                 continue
-            ptrs = []
-            for t, rows in zip(srcs, (d.M, d.N)):
-                key = (t.data_ptr(), t.stride(0), rows, d.K)
-                img = self._act_images.get(key)
-                if img is None:
-                    img = torch.empty(self.lib.phc_gemm_image_floats(rows, d.K), dtype=torch.float32, device=self.dev)
-                    self._act_images[key] = img
+            for field, t, rows, kmajor in srcs:
+                img = self.act_image(t, rows, d.K, kmajor)
+                key = (t.data_ptr(), t.stride(0), rows, d.K, kmajor)
                 if key not in jobs:
-                    jobs[key] = _lib.PhcGemmImageDesc(t.data_ptr(), t.stride(0), 0, rows, d.K, img.data_ptr())
-                ptrs.append(img.data_ptr())
-            d.A_img, d.B_img = ptrs
+                    jobs[key] = _lib.PhcGemmImageDesc(t.data_ptr(), t.stride(0), 1 if kmajor else 0, rows, d.K, img.data_ptr())
+                setattr(d, field, img.data_ptr())
         return (_lib.PhcGemmImageDesc * len(jobs))(*jobs.values()), len(jobs)
 
     def _set_mode(self) -> None:

@@ -17,7 +17,9 @@ minibatch launches again with 128 x 256 tiles (phc_gemm_tc5s_set_tile(256)).  Ea
 its weight-gradient problems alone ("dW L-k") and its input-gradient problems alone ("dX L-k").  Each group alternates A and B
 `--turns` times; a turn is `--iters` launches between two CUDA events after a warm-up.  A build that takes activation images
 (PhcGemmDesc.A_img) gets them the way MLPEngine.run_group does: one phc_gemm_make_images launch before every launch that reads
-them, inside the timed window.  Printed per group: median [min, max] us per launch
+them, inside the timed window.  A build that also takes output images (PhcGemmDesc.C_img) runs the hidden layers' forward and dX
+from the images the launch before wrote, as MLPEngine does; a build without them, and any build with 128 x 256 tiles, runs those
+problems from the fp32 activations.  Printed per group: median [min, max] us per launch
 and the TFLOP/s of tensor work (3 tensor-core products per fp32 product) for A and B, and B / A.
 
 Before any timing, the whole chain (forward, then backward) runs once per build from the same seeded workspaces, and every
@@ -45,7 +47,12 @@ class GemmDescNoImage(C.Structure):
 
 class GemmDescNoActImage(C.Structure):
     """PhcGemmDesc of a build from before the activation images (no A_img field)."""
-    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] != "A_img"]
+    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] not in ("A_img", "C_img")]
+
+
+class GemmDescNoOutImage(C.Structure):
+    """PhcGemmDesc of a build from before the epilogue's output images (no C_img field)."""
+    _fields_ = [f for f in _lib.PhcGemmDesc._fields_ if f[0] != "C_img"]
 
 
 def open_lib(path):
@@ -57,18 +64,26 @@ def open_lib(path):
     # each build gets descriptors in its own layout; one without images computes the same problems from the staged operands
     # (a build that knows A_img names it in its validation message)
     with open(path, "rb") as f:
-        act_images = b"A_img" in f.read()
-    lib.desc_type = GemmDescNoImage if not hasattr(lib, "phc_gemm_make_images") else _lib.PhcGemmDesc if act_images else GemmDescNoActImage
+        blob = f.read()
+    lib.desc_type = (GemmDescNoImage if not hasattr(lib, "phc_gemm_make_images") else GemmDescNoActImage if b"A_img" not in blob
+                     else GemmDescNoOutImage if b"C_img" not in blob else _lib.PhcGemmDesc)
     lib.phc_gemm_group.argtypes = [C.POINTER(lib.desc_type), C.c_int32, C.c_void_p]
     return lib
 
 
-def desc_array(lib, descs):
+def is_dw(d):
+    return d.accumulate and not d.a_kmajor
+
+
+def desc_array(lib, descs, out_images=True):
+    """out_images False: the problems as a build without C_img runs them (forward and dX read A from fp32 on the image loop)"""
     T = lib.desc_type
     names = [f for f, _ in T._fields_]
+    plain = "C_img" not in names or not out_images
     # without A_img a build stages the weight gradient from the fp32 operands (it refuses B_img with mn-major A)
     drop_b = lambda d: "A_img" not in names and bool(d.A_img)  # noqa: E731
-    return (T * len(descs))(*[T(*[None if f == "B_img" and drop_b(d) else getattr(d, f) for f in names]) for d in descs])
+    drop = lambda d, f: (f == "B_img" and drop_b(d)) or (plain and (f == "C_img" or (f == "A_img" and not is_dw(d))))  # noqa: E731
+    return (T * len(descs))(*[T(*[None if drop(d, f) else getattr(d, f) for f in names]) for d in descs])
 
 
 def gpu_info():
@@ -127,20 +142,25 @@ def main():
     fwd_roll = [[eng.fwd_desc(st, li, xin, ws) for st, xin, ws in roll if li < len(st.layers)] for li in range(depth)]
     groups = [(f"fwd L{li}", g) for li, g in enumerate(fwd)] + [(f"bwd L-{k + 1}", g) for k, g in enumerate(bwd)]
     groups += [(f"rollout fwd L{li} ({n_roll} rows)", g) for li, g in enumerate(fwd_roll)]
-    is_dw = lambda d: d.accumulate and not d.a_kmajor  # noqa: E731
     split = [(f"{part} L-{k + 1}", [d for d in g if is_dw(d) == (part == "dW")]) for k, g in enumerate(bwd) for part in ("dW", "dX")]
     split = [(name, g) for name, g in split if g]                  # the first layer has no dX
-    # activation images: requested by eng.bwd_descs, made by eng.make_images (it also points each dW descriptor at its images)
-    jobs = {name: eng.make_images(g) for name, g in groups + split}
-    arrays = {key: {name: (desc_array(lib, g), len(g)) for name, g in groups + split} for key, lib in libs.items()}
+    # activation images made before a launch: requested by eng.bwd_descs / eng.fwd_desc, made by eng.make_images (it also points
+    # the descriptors at them).  A build without C_img (and any build with 128 x 256 tiles, which refuse it) runs the forward and
+    # dX problems from the fp32 operands and only makes the weight gradient's images.
+    jobs = {(name, True): eng.make_images(g) for name, g in groups + split}
+    jobs.update({(name, False): eng.make_images([d for d in g if is_dw(d)]) for name, g in groups + split})
+    arrays = {(key, o): {name: (desc_array(lib, g, o), len(g)) for name, g in groups + split} for key, lib in libs.items() for o in (True, False)}
     for name, g in groups:
         assert len(g) <= _lib.PHC_GEMM_GROUP_MAX, name
 
+    tile = [128]
+
     def launch(lib, name):
-        arr, n = arrays["A" if lib is libs["A"] else "B"][name]
+        o = lib.desc_type is _lib.PhcGemmDesc and tile[0] == 128
+        arr, n = arrays[("A" if lib is libs["A"] else "B", o)][name]
         stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-        if lib.desc_type is _lib.PhcGemmDesc and jobs[name][1]:
-            rc = lib.phc_gemm_make_images(jobs[name][0], jobs[name][1], stream)
+        if lib.desc_type in (_lib.PhcGemmDesc, GemmDescNoOutImage) and jobs[(name, o)][1]:
+            rc = lib.phc_gemm_make_images(jobs[(name, o)][0], jobs[(name, o)][1], stream)
             if rc:
                 raise RuntimeError(f"phc_gemm_make_images({name}) = {rc}: {lib.phc_last_error().decode()}")
         rc = lib.phc_gemm_group(arr, n, stream)
@@ -148,6 +168,7 @@ def main():
             raise RuntimeError(f"phc_gemm_group({name}) = {rc}: {lib.phc_last_error().decode()}")
 
     def set_tile(w):
+        tile[0] = w
         for lib in libs.values():
             assert lib.phc_gemm_set_precision(_lib.PHC_GEMM_FP32_3XTF32) == 0 and lib.phc_gemm_tc5s_set_tile(w) == 0
             assert lib.phc_gemm_tc5s_set_sched(-1) == 0
@@ -208,10 +229,11 @@ def main():
 
     # ---- the activation images alone (part of B's backward times above): bytes read (the operands) and written (the images)
     if libs["B"].desc_type is _lib.PhcGemmDesc:
-        print("\nactivation images of the backward launches (B's phc_gemm_make_images alone)")
+        set_tile(128)
+        print("\nactivation images made before the launches (B's phc_gemm_make_images alone)")
         stream = C.c_void_p(torch.cuda.current_stream().cuda_stream)
         for name, _ in groups:
-            arr, n = jobs[name]
+            arr, n = jobs[(name, True)]
             if not n:
                 continue
             rd = sum(4.0 * arr[i].N * arr[i].K for i in range(n))
